@@ -72,19 +72,25 @@ struct LogAdd
 		}
 	};
 
-// builds the 17-entry table in shared memory (call with >= 17 threads, then __syncthreads)
-__device__ __forceinline__ void mb_logadd_fill(float4 *tab16)
+// builds the 17-entry table in shared memory and stores its biased base next to it (call with >= 17
+// threads, then __syncthreads)
+__device__ __forceinline__ void mb_logadd_fill(float4 *tab16, uint32_t *biased)
 	{
 	if (threadIdx.x < 17)
 		{
 		const int k = threadIdx.x;
 		tab16[k] = c_logexp1[k <= 2 ? 0 : (k <= 5 ? 1 : (k <= 9 ? 2 : 3))];
 		}
+	if (threadIdx.x == 0)
+		*biased = (uint32_t) __cvta_generic_to_shared(tab16) - (MB_LA_MAGIC_BITS << 4);
 	}
-__device__ __forceinline__ LogAdd mb_logadd_make(const float4 *tab16)
+// The biased base is READ BACK from shared memory: a value the compiler cannot see as "table address +
+// constant" stays in one register, and every LOG_ADD forms its address with one LEA.  (Computed in
+// registers, ptxas splits the bias off again and spends an IMAD plus an add per LOG_ADD.)
+__device__ __forceinline__ LogAdd mb_logadd_make(const uint32_t *biased)
 	{
-	uint32_t base = (uint32_t) __cvta_generic_to_shared(tab16) - (MB_LA_MAGIC_BITS << 4);
-	asm volatile("mov.u32 %0, %0;" : "+r"(base));          // opaque: keeps the biased base in one register
+	uint32_t base;
+	asm volatile("ld.shared.u32 %0, [%1];" : "=r"(base) : "r"((uint32_t) __cvta_generic_to_shared(biased)));
 	LogAdd la = { base };
 	return la;
 	}
@@ -153,7 +159,7 @@ struct PostParams
 	uint8_t     *rowcnt;  size_t rowcnt_stride;  // bytes
 	uint32_t     lxmax;                          // rows the scratch was sized for
 	uint32_t     fm_rows;                        // (lxmax+33): steps per strip slot in fm
-	uint32_t     cmax;                           // k_posterior_sm: columns per lane the smem state is sized for
+	uint32_t     cmax;                           // k_posterior_sm: cap on the columns per lane (<= the size class)
 	// outputs
 	uint32_t       *rowoff;         // concatenated, pair k at rowbase[k], LX+1 entries
 	const uint64_t *rowbase;

@@ -452,9 +452,7 @@ static int prepare_plan(mb200_ctx *ctx, int force_c)
 		const uint32_t LY = ctx->h_len[ctx->h_py[k]];
 		int C = force_c > 0 ? force_c : (int) std::min<uint32_t>(MB_MAX_C, (LY + 31)/32);
 		if (force_c <= 0)
-			// bins only size the shared-memory state.  14 is its own class: 4 warps x 6 arrays x 14 columns fit
-			// five CTAs in an SM's 228 KB (like 8 and 12), 16 columns only four
-			C = C <= 12 ? (C + 3)/4*4 : (C <= 14 ? 14 : 16);
+			C = mb_post_sm_class(C);          // bins only size the shared-memory state
 		bins[C].push_back(k);
 		cost[k] = (uint64_t) ctx->h_len[ctx->h_px[k]]*LY;
 		}
@@ -527,23 +525,32 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 			int smem_static = 0, occ = 0;
 			size_t smem;
 			const bool mega = ctx->mega;
+			const bool dump = dbg != nullptr;
+			const int CM = mb_post_sm_class(C);      // == C unless the width is forced
 			const int tsize = mega ? (int) ctx->mega_tsize : ctx->hmm.K*ctx->hmm.KS;
-			mb_post_sm_dispatch(mega, 2, dim3(), 0, ks, nullptr, &smem_static);
+			// the first call checks CM for all three (the occupancy query and the launch use the same CM)
+			if (!mb_post_sm_dispatch(mega, dump, CM, 2, dim3(), 0, ks, nullptr, &smem_static))
+				return mb_fail(ctx, MB200_EINVAL, "k_posterior_sm has no instantiation for size class %d", CM);
 			smem = (size_t) smem_static + (size_t)((tsize + 3) & ~3)*sizeof(float)
-			  + (size_t) MB_WARPS_PER_BLOCK*(mega ? 7 : 6)*C*32*sizeof(float);
+			  + (size_t) MB_WARPS_PER_BLOCK*(mega ? 7 : 6)*CM*32*sizeof(float);
 			if (ctx->occ_cache_k != tsize*2 + (mega ? 1 : 0))
 				{
 				memset(ctx->occ_cache, 0, sizeof ctx->occ_cache);
 				ctx->occ_cache_k = tsize*2 + (mega ? 1 : 0);
 				}
-			if (ctx->occ_cache[C] == 0)
+			if (dump)          // one pair, another instantiation: not cached
+				mb_post_sm_dispatch(mega, dump, CM, 1, dim3(), smem, ks, nullptr, &occ);
+			else
 				{
-				mb_post_sm_dispatch(mega, 1, dim3(), smem, ks, nullptr, &occ);
-				ctx->occ_cache[C] = occ;
+				if (ctx->occ_cache[C] == 0)
+					{
+					mb_post_sm_dispatch(mega, dump, CM, 1, dim3(), smem, ks, nullptr, &occ);
+					ctx->occ_cache[C] = occ;
+					}
+				occ = ctx->occ_cache[C];
 				}
-			occ = ctx->occ_cache[C];
 			if (occ <= 0)
-				return mb_fail(ctx, MB200_ECUDA, "k_posterior_sm (CM=%d) cannot be resident (smem %zu)", C, smem);
+				return mb_fail(ctx, MB200_ECUDA, "k_posterior_sm (CM=%d) cannot be resident (smem %zu)", CM, smem);
 			uint32_t nblocks = (uint32_t) occ*ctx->prop.multiProcessorCount;
 			const uint32_t need_blocks = ((uint32_t) b.size() + MB_WARPS_PER_BLOCK - 1)/MB_WARPS_PER_BLOCK;
 			nblocks = std::max(1u, std::min(nblocks, need_blocks));
@@ -604,7 +611,7 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 				P.dbg_fwd = dbg->fwd; P.dbg_bwd = dbg->bwd; P.dbg_post = dbg->post; P.dbg_total = dbg->total;
 				}
 			P.cmax = (uint32_t) C;
-			mb_post_sm_dispatch(mega, 0, dim3(nblocks), smem, ks, &P, nullptr);
+			mb_post_sm_dispatch(mega, dump, CM, 0, dim3(nblocks), smem, ks, &P, nullptr);
 			CU(cudaGetLastError());
 			ctx->stats.kernel_launches++;
 			}

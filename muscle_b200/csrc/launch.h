@@ -3,6 +3,15 @@
 #include "common.cuh"
 
 #define MB_MAX_C 16
-// k_posterior_sm (state in shared memory, runtime columns-per-lane)
-// op 0: launch, 1: occupancy (blocks/SM) -> *out, 2: static smem struct bytes -> *out
-bool mb_post_sm_dispatch(bool mega, int op, dim3 grid, size_t smem, cudaStream_t st, const PostParams *P, int *out);
+// k_posterior_sm is compiled per shared-memory size class CM (columns per lane): 4, 8, 12, 14, 16.
+// 14 is its own class: 4 warps x 6 words x 14 columns fit five CTAs in an SM's 228 KB (like 8 and
+// 12), 16 columns only four.  Any C <= 16 runs in the smallest class that holds it.
+static inline int mb_post_sm_class(int C)
+	{
+	return C <= 12 ? (C + 3)/4*4 : (C <= 14 ? 14 : 16);
+	}
+// op 0: launch, 1: occupancy (blocks/SM) -> *out, 2: static smem struct bytes -> *out.
+// dump: the instantiation that writes the dense debug arrays of PostParams (mb200_calc_post_dense).
+// Returns false if cm is not a size class.
+bool mb_post_sm_dispatch(bool mega, bool dump, int cm, int op, dim3 grid, size_t smem, cudaStream_t st,
+  const PostParams *P, int *out);

@@ -7,15 +7,17 @@
 // (calcalnscoreflat.cpp:4-32) of the reference.
 //
 // Mapping.  One warp owns one pair at a time (persistent warps pull pairs, longest first, from an
-// atomic cursor).  Lane l owns C consecutive DP columns of Y (C = ceil(LY/32), a runtime value); a
-// warp therefore covers a strip of 32*C columns and longer Y are processed strip after strip with
-// the strip-edge column handed over through a small per-warp buffer.  Rows of X are swept in
-// anti-diagonal (wavefront) order: at step t lane l works on row t-l, the cell to the left lives in
-// lane l-1 and was produced one step earlier, so the recurrence dependency is a few warp shuffles
-// per step.  The per-column wavefront state lives in SHARED MEMORY as [c][lane] arrays (bank ==
-// lane, conflict free) and the loop over the lane's columns is rolled: the hot loops are short and
-// stay in the instruction cache (a register-resident, fully unrolled variant stalls on instruction
-// fetch).  Only the
+// atomic cursor).  Lane l owns C consecutive DP columns of Y (C = ceil(LY/32) capped at the size
+// class CM, a compile-time parameter); a warp therefore covers a strip of 32*C columns and longer Y
+// are processed strip after strip with the strip-edge column handed over through a small per-warp
+// buffer.  Rows of X are swept in anti-diagonal (wavefront) order: at step t lane l works on row t-l,
+// the cell to the left lives in lane l-1 and was produced one step earlier, so the recurrence
+// dependency is a few warp shuffles per step.  The per-column wavefront state lives in SHARED MEMORY,
+// one record per (column, lane) stored [c][lane] (lane-contiguous: conflict free): {S, M, IX, JX} as
+// one float4 and {class of Y, insert emission of Y} as one 64-bit word, so that a column costs one
+// 128-bit load and store of state, one 64-bit load of its Y data and pointers that move by constants.
+// The loop over the lane's columns is rolled: the hot loops are short and stay in the instruction
+// cache (a register-resident, fully unrolled variant stalls on instruction fetch).  Only the
 // Forward M-state is spilled (4 B/cell), in [step][c][lane] order so that both the Forward write
 // and the Backward read are full 128-byte lines.  Backward walks the same anti-diagonals in
 // reverse, fuses the Fwd (*) Bwd posterior, thresholds at log(0.01) and appends survivors to a
@@ -28,7 +30,11 @@
 // so the reference's border formulas (first row/column of Forward, fwdflat3.cpp:35-93; last
 // row/column of Backward, bwdflat3.cpp:132-176) fall out of the general cell update when the
 // out-of-range neighbours are LOG_ZERO.  The only injected values are the start scores at Forward
-// (0,0) and the end scores at Backward (LX,LY) (bwdflat3.cpp:53-61).
+// (0,0) and the end scores at Backward (LX,LY) (bwdflat3.cpp:53-61).  Columns past LY (the tail of
+// the lane that holds column LY in the last strip) are never computed: Forward never flows back from
+// them, and in Backward they would stay exactly LOG_ZERO, the value they are initialised to.  So the
+// cell (LX,LY) is the last cell of its lane's row in Forward (read out after the loop) and the first
+// in Backward (set before the loop), and the hot loops carry no test for either.
 //
 // Emissions.  Plain mode: residue classes index a K x K match table and a K-entry insert table
 // (PairHMM::m_MatchScore / m_InsScore, pairhmm.h:26-29).  MEGA mode (Muscle-3D feature profiles,
@@ -38,10 +44,13 @@
 // mega.cpp:340-359) -- the products are formed once on the host (same fp32 multiply), the kernel adds
 // them in order -- and the insert emission is a per-position value precomputed the same way
 // (Mega::GetInsScore, mega.cpp:273-286).  Same recurrences, same kernel, one template flag.
+//
+// DUMP: the instantiation used by mb200_calc_post_dense also writes the dense Forward-M, Backward-M,
+// posterior and total of its pair; production launches carry no dump code.
 #pragma once
 #include "common.cuh"
 
-#define MB_SM_ARRAYS 6            // S/old, M, IX, JX, ycode, eY  (+1 in MEGA mode: second word of feature letters)
+#define MB_SM_ARRAYS 6            // words of state per (column, lane): float4 state + {ycode, eY}  (+1 in MEGA mode: letters 4..7)
 #ifndef MB_SM_BLOCKS
 #define MB_SM_BLOCKS 5            // resident CTAs/SM the register budget is tuned for (64K registers: <= 102 per thread)
 #endif
@@ -53,8 +62,9 @@
 
 struct PostSmemHdr
 	{
-	float4 coef[17];      // LOGEXP1 pieces indexed by ceil(2*gap), see LogAdd
-	float  insT[MB_MAX_K];
+	float4   coef[17];    // LOGEXP1 pieces indexed by ceil(2*gap), see LogAdd
+	float    insT[MB_MAX_K];
+	uint32_t labase;      // biased shared address of coef (mb_logadd_make)
 	};
 
 // sum over features of the pre-multiplied pair tables, in feature order starting from 0
@@ -72,7 +82,8 @@ __device__ __forceinline__ float mb_mega_emit(const float *T, const uint32_t (&x
 	return e;
 	}
 
-template <bool MEGA>
+// CM: size class (columns per lane the shared memory is sized for; P.cmax <= CM caps C at run time)
+template <bool MEGA, int CM, bool DUMP>
 __global__ void __launch_bounds__(32*MB_WARPS_PER_BLOCK, MEGA ? 4 : MB_SM_BLOCKS)
 k_posterior_sm(const PostParams P)
 	{
@@ -83,20 +94,15 @@ k_posterior_sm(const PostParams P)
 	const int lane = threadIdx.x & 31;
 	const int wib = threadIdx.x >> 5;
 	const int gwarp = blockIdx.x*MB_WARPS_PER_BLOCK + wib;
-	const int CM = (int) P.cmax;                             // columns per lane the smem is sized for
 	float *matchT = reinterpret_cast<float *>(smem_raw + sizeof(PostSmemHdr));
 	const int tsize = MEGA ? (int) P.mega_tsize : h.K*h.KS;
 	float *wbase = matchT + ((tsize + 3) & ~3) + (size_t) wib*NARR*CM*32;
-	float *aS = wbase;                  // Forward: S ; EA: old row
-	float *aM = aS + CM*32;             // M        ; EA: staged posterior row (column-linear)
-	float *aIX = aM + CM*32;            //          ; EA: lane-local prefix maxima
-	float *aJX = aIX + CM*32;
-	int   *aY = reinterpret_cast<int *>(aJX + CM*32);
-	float *aE = reinterpret_cast<float *>(aY) + CM*32;
-	int   *aY2 = reinterpret_cast<int *>(aE + CM*32);       // MEGA only: letters of features 4..7
-	(void) aY2;
+	float4   *st = reinterpret_cast<float4 *>(wbase);                  // Forward {S, M, IX, JX}; Backward {M, IX, JX, -}
+	uint2    *ye = reinterpret_cast<uint2 *>(wbase + 4*CM*32);         // {class (MEGA: letters 0..3), bits of eY}
+	uint32_t *y2 = reinterpret_cast<uint32_t *>(wbase + 6*CM*32);      // MEGA only: letters 4..7
+	(void) y2;
 
-	mb_logadd_fill(sm.coef);
+	mb_logadd_fill(sm.coef, &sm.labase);
 	if (!MEGA)
 		for (int k = threadIdx.x; k < h.K; k += blockDim.x)
 			sm.insT[k] = P.insT[k];
@@ -105,7 +111,7 @@ k_posterior_sm(const PostParams P)
 	const int nf = (int) P.mega_nf;
 	__syncthreads();
 
-	const LogAdd la = mb_logadd_make(sm.coef);
+	const LogAdd la = mb_logadd_make(&sm.labase);
 	const float Z = MB_LOG_ZERO;
 
 	float       *fm     = P.fm + (size_t) gwarp*P.fm_stride;
@@ -133,7 +139,7 @@ k_posterior_sm(const PostParams P)
 		const float *Xi = P.insT + P.seqoff[sx];
 		const float *Yi = P.insT + P.seqoff[sy];
 		(void) Xc; (void) Yc; (void) Xl; (void) Yl; (void) Xi; (void) Yi;
-		const int C = min(CM, (LY + 31) >> 5);            // columns per lane for this pair
+		const int C = min(min(CM, (int) P.cmax), (LY + 31) >> 5);   // columns per lane for this pair
 		const int W = 32*C;
 		const int nstrips = (LY + W - 1)/W;
 		const int lastj0 = (nstrips - 1)*W;
@@ -151,6 +157,7 @@ k_posterior_sm(const PostParams P)
 			const int ncol = min(W, LY - j0);
 			const int nl = (ncol + C - 1)/C;
 			const bool last = (strip == nstrips - 1);
+			const int cn = (last && lane == lcl) ? clast + 1 : C;     // columns of this lane up to LY
 			const float4 *edgeIn = (strip & 1) ? edge0 : edge1;
 			float4 *edgeOut = (strip & 1) ? edge1 : edge0;
 			float *fms = fm + (size_t) strip*P.fm_rows*W;
@@ -161,17 +168,15 @@ k_posterior_sm(const PostParams P)
 				if (MEGA)
 					{
 					const uint2 yl = jj < LY ? Yl[jj] : make_uint2(0u, 0u);
-					aY[c*32 + lane] = (int) yl.x;
-					aY2[c*32 + lane] = (int) yl.y;
-					aE[c*32 + lane] = jj < LY ? Yi[jj] : 0.0f;
+					ye[c*32 + lane] = make_uint2(yl.x, __float_as_uint(jj < LY ? Yi[jj] : 0.0f));
+					y2[c*32 + lane] = yl.y;
 					}
 				else
 					{
 					const int code = jj < LY ? (int) Yc[jj] : h.pad;
-					aY[c*32 + lane] = code;
-					aE[c*32 + lane] = sm.insT[code];
+					ye[c*32 + lane] = make_uint2((uint32_t) code, __float_as_uint(sm.insT[code]));
 					}
-				aS[c*32 + lane] = Z; aM[c*32 + lane] = Z; aIX[c*32 + lane] = Z; aJX[c*32 + lane] = Z;
+				st[c*32 + lane] = make_float4(Z, Z, Z, Z);
 				}
 			float outM = Z, outAIY = Z, outAJY = Z, outS = Z;
 			float dprev = Z;
@@ -234,6 +239,7 @@ k_posterior_sm(const PostParams P)
 					float diag = dprev;
 					dprev = Ls;
 					float lm = Lm, laiy = Laiy, lajy = Lajy, sLast = Z;
+					float ix = Z, jx = Z, iy = Z, jy = Z;
 					const float *mrow = matchT + (MEGA ? 0 : xc*h.KS);
 					uint32_t xb[8];
 					if (MEGA)
@@ -242,40 +248,38 @@ k_posterior_sm(const PostParams P)
 						for (int f = 0; f < 8; ++f)
 							xb[f] = P.mega_base[f] + ((f < 4 ? (xl.x >> (8*f)) : (xl.y >> (8*(f - 4)))) & 255u)*P.mega_alpha[f];
 						}
-					const bool cap = last && i == LX && lane == lcl;
+					float4 *sp = st + lane;
+					const uint2 *yp = ye + lane;
+					const uint32_t *y2p = y2 + lane;
 					float *dst = fms + (size_t) t*W + lane;
-					const bool dump = P.dbg_fwd != nullptr && i >= 1;
+					(void) y2p;
 MB_UNROLL(MB_SM_UNROLL)
-					for (int c = 0; c < C; ++c)
+					for (int c = 0; c < cn; ++c, sp += 32, yp += 32, y2p += 32, dst += 32)
 						{
-						const int o = c*32 + lane;
-						const float Mo = aM[o], IXo = aIX[o], JXo = aJX[o];
-						const float eyc = aE[o];
-						const float em = MEGA ? mb_mega_emit(matchT, xb, (uint32_t) aY[o], (uint32_t) aY2[o], nf) : mrow[aY[o]];
+						const float4 v = *sp;                      // {S, M, IX, JX} of row i-1
+						const uint2 y = *yp;
+						const float eyc = __uint_as_float(y.y);
+						const float em = MEGA ? mb_mega_emit(matchT, xb, y.x, *y2p, nf) : mrow[y.x];
 						const float m = ADD(diag, em);
-						const float ix = ADD(la(ADD(IXo, h.tII), ADD(Mo, h.tMI)), ex);
-						const float jx = ADD(la(ADD(JXo, h.tJJ), ADD(Mo, h.tMJ)), ex);
-						const float iy = ADD(la(laiy, ADD(lm, h.tMI)), eyc);
-						const float jy = ADD(la(lajy, ADD(lm, h.tMJ)), eyc);
+						ix = ADD(la(ADD(v.z, h.tII), ADD(v.y, h.tMI)), ex);
+						jx = ADD(la(ADD(v.w, h.tJJ), ADD(v.y, h.tMJ)), ex);
+						iy = ADD(la(laiy, ADD(lm, h.tMI)), eyc);
+						jy = ADD(la(lajy, ADD(lm, h.tMJ)), eyc);
 						const float s = la(ADD(m, h.tMM), la(ADD(ix, h.tIM), la(ADD(jx, h.tJM),
 						  la(ADD(iy, h.tIM), ADD(jy, h.tJM)))));
-						diag = aS[o];
-						aS[o] = s; aM[o] = m; aIX[o] = ix; aJX[o] = jx;
+						diag = v.x;
+						*sp = make_float4(s, m, ix, jx);
 						lm = m;
 						laiy = ADD(iy, h.tII);
 						lajy = ADD(jy, h.tJJ);
 						sLast = s;
-						dst[c*32] = m;
-						if (cap && c == clast)
-							{
-							fin0 = m; fin1 = ix; fin2 = iy; fin3 = jx; fin4 = jy;
-							}
-						if (dump)
-							{
-							const int col = j0 + lane*C + c;
-							if (col < LY)
-								P.dbg_fwd[(size_t)(i - 1)*LY + col] = m;
-							}
+						*dst = m;
+						if (DUMP && i >= 1)
+							P.dbg_fwd[(size_t)(i - 1)*LY + j0 + lane*C + c] = m;
+						}
+					if (last && i == LX && lane == lcl)    // cell (LX,LY) is the lane's last
+						{
+						fin0 = lm; fin1 = ix; fin2 = iy; fin3 = jx; fin4 = jy;
 						}
 					outM = lm; outAIY = laiy; outAJY = lajy; outS = sLast;
 					if (lane == 31 && !last)
@@ -297,7 +301,7 @@ MB_UNROLL(MB_SM_UNROLL)
 		total = la(total, ADD(fin2, h.tSI));
 		total = la(total, ADD(fin3, h.tSJ));
 		total = la(total, ADD(fin4, h.tSJ));
-		if (P.dbg_total != nullptr && lane == 0)
+		if (DUMP && lane == 0)
 			*P.dbg_total = total;
 
 		// ============================ Backward + posterior ============================
@@ -309,6 +313,7 @@ MB_UNROLL(MB_SM_UNROLL)
 			const int ncol = min(W, LY - j0);
 			const int nl = (ncol + C - 1)/C;
 			const bool last = (strip == nstrips - 1);
+			const int cn = (last && lane == lcl) ? clast + 1 : C;     // columns of this lane up to LY
 			const float4 *edgeIn = (strip & 1) ? edge0 : edge1;
 			float4 *edgeOut = (strip & 1) ? edge1 : edge0;
 			const float *fms = fm + (size_t) strip*P.fm_rows*W;
@@ -319,17 +324,15 @@ MB_UNROLL(MB_SM_UNROLL)
 				if (MEGA)
 					{
 					const uint2 yl = jj < LY ? Yl[jj] : make_uint2(0u, 0u);
-					aY[c*32 + lane] = (int) yl.x;
-					aY2[c*32 + lane] = (int) yl.y;
-					aE[c*32 + lane] = jj < LY ? Yi[jj] : 0.0f;
+					ye[c*32 + lane] = make_uint2(yl.x, __float_as_uint(jj < LY ? Yi[jj] : 0.0f));
+					y2[c*32 + lane] = yl.y;
 					}
 				else
 					{
 					const int code = jj < LY ? (int) Yc[jj] : h.pad;
-					aY[c*32 + lane] = code;
-					aE[c*32 + lane] = sm.insT[code];
+					ye[c*32 + lane] = make_uint2((uint32_t) code, __float_as_uint(sm.insT[code]));
 					}
-				aM[c*32 + lane] = Z; aIX[c*32 + lane] = Z; aJX[c*32 + lane] = Z;
+				st[c*32 + lane] = make_float4(Z, Z, Z, Z);
 				}
 			float outM = Z, outIY = Z, outJY = Z;
 			float dprev = Z;
@@ -382,64 +385,80 @@ MB_UNROLL(MB_SM_UNROLL)
 					const uint32_t cnt0 = cnt;
 					mb200_entry *row = rows + (size_t)(i - 1)*MB_CAP;
 					const int t = i + lane;
-					const float *src = fms + (size_t) t*W + lane;
+					const int col0 = j0 + lane*C;
 					float mdiag = dprev;
 					dprev = Rm;
 					float riy = Riy, rjy = Rjy, mFirst = Z;
-					const bool inj = last && i == LX && lane == lcl;
-					const bool dump = P.dbg_bwd != nullptr;
-					float fmNext = src[(C - 1)*32];
-MB_UNROLL(MB_SM_UNROLL)
-					for (int c = C - 1; c >= 0; --c)
+					// posterior (calcposteriorflat.cpp:14-22); candidates arrive with descending column
+					auto post = [&](int c, float fmv, float m)
 						{
-						const int o = c*32 + lane;
-						const float fmv = fmNext;
-						if (c > 0)
-							fmNext = src[(c - 1)*32];
-						const float Mo = aM[o], IXo = aIX[o], JXo = aJX[o];
-						const float eyc = aE[o];
-						const float em = MEGA ? mb_mega_emit(matchT, xb, (uint32_t) aY[o], (uint32_t) aY2[o], nf) : mrow[aY[o]];
-						const float nM = ADD(mdiag, em);
-						const float nIX = ADD(IXo, ex);
-						const float nJX = ADD(JXo, ex);
-						const float nIY = ADD(riy, eyc);
-						const float nJY = ADD(rjy, eyc);
-						float m = la(ADD(h.tMM, nM), la(ADD(h.tMI, nIX), la(ADD(h.tMJ, nJX),
-						  la(ADD(h.tMI, nIY), ADD(h.tMJ, nJY)))));
-						float ix = la(ADD(h.tII, nIX), ADD(h.tIM, nM));
-						float jx = la(ADD(h.tJJ, nJX), ADD(h.tJM, nM));
-						float iy = la(ADD(h.tII, nIY), ADD(h.tIM, nM));
-						float jy = la(ADD(h.tJJ, nJY), ADD(h.tJM, nM));
-						if (inj && c == clast)
-							{
-							m = h.tSM; ix = h.tSI; jx = h.tSJ; iy = h.tSI; jy = h.tSJ;
-							}
-						mdiag = Mo;
-						aM[o] = m; aIX[o] = ix; aJX[o] = jx;
-						riy = iy; rjy = jy;
-						mFirst = m;
-						// posterior (calcposteriorflat.cpp:14-22); candidates arrive with descending column
-						const int col = j0 + lane*C + c;
 						const float score = __fsub_rn(ADD(fmv, m), total);
-						if (col < LY && score >= h.minScore)
+						if (score >= h.minScore)
 							{
 							const float p = score >= 0.0f ? 1.0f : mb_expf_glibc(score);
 							if (cnt < MB_CAP)
 								{
 								row[cnt].p = p;
-								row[cnt].col = (uint32_t) col;
+								row[cnt].col = (uint32_t)(col0 + c);
 								}
 							else
 								overflow = true;
 							++cnt;
 							kept += (p >= 0.01f) ? 1u : 0u;
 							}
-						if (dump && col < LY)
+						if (DUMP)
 							{
-							P.dbg_bwd[(size_t)(i - 1)*LY + col] = m;
-							P.dbg_post[(size_t)(i - 1)*LY + col] =
+							P.dbg_bwd[(size_t)(i - 1)*LY + col0 + c] = m;
+							P.dbg_post[(size_t)(i - 1)*LY + col0 + c] =
 							  score < h.minScore ? 0.0f : (score >= 0.0f ? 1.0f : mb_expf_glibc(score));
 							}
+						};
+					float4 *sp = st + lane;
+					const uint2 *yp = ye + lane;
+					const uint32_t *y2p = y2 + lane;
+					const float *src = fms + (size_t) t*W + lane;     // Forward M of the lane's column 0
+					(void) y2p;
+					int c = cn - 1;
+					sp += c*32; yp += c*32; y2p += c*32; src += c*32;
+					if (last && i == LX && lane == lcl)
+						{
+						// cell (LX,LY), the lane's first: the end scores (bwdflat3.cpp:53-61)
+						mdiag = sp->x;
+						*sp = make_float4(h.tSM, h.tSI, h.tSJ, Z);
+						riy = h.tSI; rjy = h.tSJ; mFirst = h.tSM;
+						post(c, *src, h.tSM);
+						--c; sp -= 32; yp -= 32; y2p -= 32; src -= 32;
+						}
+					// the prefetch reads src[-32] when c reaches 0, unguarded: it is inside this warp's spill (t >= 1),
+					// and since t is the same in every lane it is step t-1's column C-1, the line this warp loads
+					// first in its next step, so it adds no line of traffic
+					float fmNext = *src;
+MB_UNROLL(MB_SM_UNROLL)
+					for (; c >= 0; --c, sp -= 32, yp -= 32, y2p -= 32)
+						{
+						const float fmv = fmNext;
+						src -= 32;
+						fmNext = *src;
+						const float4 v = *sp;                      // {M, IX, JX, -} of row i+1
+						const uint2 y = *yp;
+						const float eyc = __uint_as_float(y.y);
+						const float em = MEGA ? mb_mega_emit(matchT, xb, y.x, *y2p, nf) : mrow[y.x];
+						const float nM = ADD(mdiag, em);
+						const float nIX = ADD(v.y, ex);
+						const float nJX = ADD(v.z, ex);
+						const float nIY = ADD(riy, eyc);
+						const float nJY = ADD(rjy, eyc);
+						const float m = la(ADD(h.tMM, nM), la(ADD(h.tMI, nIX), la(ADD(h.tMJ, nJX),
+						  la(ADD(h.tMI, nIY), ADD(h.tMJ, nJY)))));
+						const float ix = la(ADD(h.tII, nIX), ADD(h.tIM, nM));
+						const float jx = la(ADD(h.tJJ, nJX), ADD(h.tJM, nM));
+						const float iy = la(ADD(h.tII, nIY), ADD(h.tIM, nM));
+						const float jy = la(ADD(h.tJJ, nJY), ADD(h.tJM, nM));
+						mdiag = v.x;
+						*sp = make_float4(m, ix, jx, Z);
+						riy = iy; rjy = jy;
+						mFirst = m;
+						post(c, fmv, m);
 						}
 					outM = mFirst; outIY = riy; outJY = rjy;
 					if (lane == 0 && strip > 0)
@@ -474,9 +493,10 @@ MB_UNROLL(MB_SM_UNROLL)
 
 		float eaScore = 0.0f;
 		{
-		float *old = aS;            // [c][lane]
-		float *rowbuf = aM;         // column-linear: [lane*C + c]
-		float *pre = aIX;           // [c][lane]
+		// the warp's state area, reused as three plain float arrays of CM*32
+		float *old = wbase;                 // [c][lane]
+		float *rowbuf = wbase + CM*32;      // column-linear: [lane*C + c]
+		float *pre = wbase + 2*CM*32;       // [c][lane]
 		float *eIn = reinterpret_cast<float *>(edge0);
 		float *eOut = reinterpret_cast<float *>(edge1);
 		uint32_t written = 0;
