@@ -13,7 +13,9 @@
 #define MB_LOG_ZERO (-2e20f)          // scoretype.h:89
 #define MB_MAX_K 64                    // residue classes the smem tables can hold
 #define MB_CAP MB200_MAX_ROW_NNZ       // candidate entries per posterior row
-#define MB_WARPS_PER_BLOCK 4            // posterior kernel: warps (pairs in flight) per CTA
+#define MB_WARPS_PER_BLOCK 4            // posterior kernel: warps (chains in flight) per CTA
+#define MB_CHAIN_MAX 32                 // posterior kernel: pairs in one chain (one per lane when the chain is read)
+#define MB_CHAIN_BUF (MB_CHAIN_MAX*38)  // words of per-warp chain scratch: kept counts [pair][lane], totals [pair], final cells [pair][5]
 
 struct MbHmm
 	{
@@ -149,15 +151,17 @@ struct PostParams
 	const uint64_t *seqoff;
 	const uint32_t *seqlen;
 	const uint32_t *px, *py;        // store pair -> sequence ids
-	const uint32_t *order;          // work list (store pair ids), longest first
-	uint32_t nwork;
+	const uint32_t *order;          // store pair ids, chain after chain
+	const uint32_t *chain;          // work list: chain w is order[chain[w] .. chain[w+1]), longest first
+	uint32_t nwork;                 // chains
 	uint32_t *counter;              // work-stealing cursor for this launch
 	// per-warp scratch
 	float       *fm;      size_t fm_stride;      // floats
 	float4      *edge;    size_t edge_stride;    // float4, two ping-pong halves
 	mb200_entry *rows;    size_t rows_stride;    // entries
 	uint8_t     *rowcnt;  size_t rowcnt_stride;  // bytes
-	uint32_t     lxmax;                          // rows the scratch was sized for
+	uint32_t    *chainbuf;                       // MB_CHAIN_BUF words per warp
+	uint32_t     lxmax;                          // rows of one pair the scratch was sized for
 	uint32_t     fm_rows;                        // (lxmax+33): steps per strip slot in fm
 	uint32_t     cmax;                           // k_posterior_sm: cap on the columns per lane (<= the size class)
 	// outputs

@@ -65,6 +65,7 @@ void mb_release_post_scratch(mb200_ctx *ctx)
 	for (int c = 0; c <= MB_MAX_C; ++c)
 		{
 		ctx->d_fm[c].release(); ctx->d_edge[c].release(); ctx->d_rows[c].release(); ctx->d_rowcnt[c].release();
+		ctx->d_chainbuf[c].release();
 		}
 	}
 
@@ -131,7 +132,7 @@ void mb200_destroy(mb200_ctx *ctx)
 	cudaSetDevice(ctx->device);
 	cudaStreamSynchronize(ctx->stream);
 	DevBuf *bufs[] = { &ctx->d_matchT, &ctx->d_insT, &ctx->d_codes, &ctx->d_seqoff, &ctx->d_seqlen, &ctx->d_px,
-	  &ctx->d_py, &ctx->d_order,
+	  &ctx->d_py, &ctx->d_order, &ctx->d_chain,
 	  &ctx->d_rowoff, &ctx->d_rowbase, &ctx->d_entries, &ctx->d_cursor, &ctx->d_entbase, &ctx->d_nnz,
 	  &ctx->d_ea, &ctx->d_dbg, &ctx->d_pack_off, &ctx->d_pack_ent, &ctx->d_entries2,
 	  &ctx->d_tr_rowoff, &ctx->d_tr_rowbase, &ctx->d_tr_entries, &ctx->d_tr_entbase, &ctx->d_tr_perm,
@@ -398,6 +399,11 @@ int mb200_set_seqs_mega(mb200_ctx *ctx, uint32_t nseq, const uint8_t *letters, c
 
 // ------------------------------------------------------------------------------------------
 // posterior stage
+// A work unit of k_posterior_sm is a chain of pairs that share Y; the warp's wavefront fills and
+// drains once per chain.  kChainRows bounds a chain's Forward rows (sum of LX+2) and so the per-warp
+// Forward-M spill and candidate rows: at 1280 the C3 workload (1000 proteins of ~350 residues) runs
+// chains of about 3.5 pairs and its scratch stays a small part of one 80 GB device.
+static const uint64_t kChainRows = 1280;
 // Plan = everything that depends only on the pair list: per-pair row bases, the column-width
 // bins and the longest-first work order.  Cached across calls with the same pair list so that a
 // repeated mb200_posteriors_allpairs() moves no host data.
@@ -443,10 +449,9 @@ static int prepare_plan(mb200_ctx *ctx, int force_c)
 	CU(cudaMemcpyAsync(ctx->d_rowbase.p, rowbase.data(), (np + 1)*sizeof(uint64_t), cudaMemcpyHostToDevice, st));
 	ctx->stats.h2d_bytes += 2ull*np*sizeof(uint32_t) + (np + 1)*sizeof(uint64_t);
 
-	// bin pairs by C = columns per lane; inside a bin most cells first
+	// bin pairs by C = columns per lane
 	auto &bins = ctx->plan_bins;
 	bins.assign(MB_MAX_C + 1, std::vector<uint32_t>());
-	std::vector<uint64_t> cost(np);
 	for (uint32_t k = 0; k < np; ++k)
 		{
 		const uint32_t LY = ctx->h_len[ctx->h_py[k]];
@@ -454,26 +459,58 @@ static int prepare_plan(mb200_ctx *ctx, int force_c)
 		if (force_c <= 0)
 			C = mb_post_sm_class(C);          // bins only size the shared-memory state
 		bins[C].push_back(k);
-		cost[k] = (uint64_t) ctx->h_len[ctx->h_px[k]]*LY;
 		}
-	std::vector<uint32_t> order;
+	// inside a bin, pairs with the same Y form chains (store order, at most kChainRows Forward rows and
+	// MB_CHAIN_MAX pairs; pairs that need more than one strip stay alone); most cells first
+	std::vector<uint32_t> order, chain;
 	order.reserve(np);
 	ctx->plan_bin_start.assign(MB_MAX_C + 2, 0);
 	ctx->plan_lxmax.assign(MB_MAX_C + 1, 0);
 	ctx->plan_lymax.assign(MB_MAX_C + 1, 0);
+	ctx->plan_fmax.assign(MB_MAX_C + 1, 0);
+	ctx->plan_rmax.assign(MB_MAX_C + 1, 0);
+	std::vector<int> open(ctx->nseq, -1);
 	for (int C = 1; C <= MB_MAX_C; ++C)
 		{
-		auto &b = bins[C];
-		std::stable_sort(b.begin(), b.end(), [&](uint32_t a, uint32_t c2) { return cost[a] > cost[c2]; });
-		ctx->plan_bin_start[C] = (uint32_t) order.size();
-		order.insert(order.end(), b.begin(), b.end());
-		for (uint32_t k : b)
+		std::vector<std::vector<uint32_t>> chains;
+		std::vector<uint64_t> frows, cost;
+		for (uint32_t k : bins[C])
 			{
-			ctx->plan_lxmax[C] = std::max(ctx->plan_lxmax[C], ctx->h_len[ctx->h_px[k]]);
-			ctx->plan_lymax[C] = std::max(ctx->plan_lymax[C], ctx->h_len[ctx->h_py[k]]);
+			const uint32_t x = ctx->h_px[k], y = ctx->h_py[k];
+			const uint32_t LX = ctx->h_len[x], LY = ctx->h_len[y];
+			int &c = open[y];
+			if (c < 0 || LY > 32u*C || frows[c] + LX + 2 > kChainRows || chains[c].size() == MB_CHAIN_MAX)
+				{
+				c = (int) chains.size();
+				chains.emplace_back();
+				frows.push_back(0);
+				cost.push_back(0);
+				}
+			chains[c].push_back(k);
+			frows[c] += LX + 2;
+			cost[c] += (uint64_t) LX*LY;
+			ctx->plan_lxmax[C] = std::max(ctx->plan_lxmax[C], LX);
+			ctx->plan_lymax[C] = std::max(ctx->plan_lymax[C], LY);
+			ctx->plan_fmax[C] = std::max<uint64_t>(ctx->plan_fmax[C], frows[c]);
+			ctx->plan_rmax[C] = std::max<uint64_t>(ctx->plan_rmax[C], frows[c] - 2*chains[c].size());
+			}
+		for (uint32_t k : bins[C])
+			open[ctx->h_py[k]] = -1;
+		std::vector<uint32_t> idx(chains.size());
+		std::iota(idx.begin(), idx.end(), 0u);
+		std::stable_sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return cost[a] > cost[b]; });
+		ctx->plan_bin_start[C] = (uint32_t) chain.size();
+		for (uint32_t c : idx)
+			{
+			chain.push_back((uint32_t) order.size());
+			order.insert(order.end(), chains[c].begin(), chains[c].end());
 			}
 		}
-	ctx->plan_bin_start[MB_MAX_C + 1] = (uint32_t) order.size();
+	ctx->plan_bin_start[MB_MAX_C + 1] = (uint32_t) chain.size();
+	chain.push_back((uint32_t) order.size());
+	ENSURE(ctx->d_chain, chain.size()*sizeof(uint32_t));
+	CU(cudaMemcpyAsync(ctx->d_chain.p, chain.data(), chain.size()*sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+	ctx->stats.h2d_bytes += chain.size()*sizeof(uint32_t);
 	CU(cudaMemcpyAsync(ctx->d_order.p, order.data(), np*sizeof(uint32_t), cudaMemcpyHostToDevice, st));
 	CU(cudaStreamSynchronize(st));     // host vectors above go out of scope
 	ctx->stats.h2d_bytes += np*sizeof(uint32_t);
@@ -552,32 +589,37 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 			if (occ <= 0)
 				return mb_fail(ctx, MB200_ECUDA, "k_posterior_sm (CM=%d) cannot be resident (smem %zu)", CM, smem);
 			uint32_t nblocks = (uint32_t) occ*ctx->prop.multiProcessorCount;
-			const uint32_t need_blocks = ((uint32_t) b.size() + MB_WARPS_PER_BLOCK - 1)/MB_WARPS_PER_BLOCK;
+			const uint32_t nchains = bin_start[C + 1] - bin_start[C];
+			const uint32_t need_blocks = (nchains + MB_WARPS_PER_BLOCK - 1)/MB_WARPS_PER_BLOCK;
 			nblocks = std::max(1u, std::min(nblocks, need_blocks));
 			const size_t nwarps = (size_t) nblocks*MB_WARPS_PER_BLOCK;
 			// scratch geometry; shrink the resident warp count if the Forward-M spill would not fit
 			PostParams P;
 			memset(&P, 0, sizeof P);
 			P.lxmax = lxmax;
+			// Forward-M spill: a strip slot of fm_rows steps per strip of a single pair, or the steps of
+			// a chain (at most its Forward rows + 30), which always has one strip
 			P.fm_rows = lxmax + 33;
-			P.fm_stride = (size_t) nstrips*P.fm_rows*W;
+			P.fm_stride = std::max<size_t>((size_t) nstrips*P.fm_rows, ctx->plan_fmax[C] + 31)*W;
 			P.edge_stride = 2*((size_t) lxmax + 2);
-			P.rows_stride = (size_t) lxmax*MB_CAP;
-			P.rowcnt_stride = ((size_t) lxmax + 31)/16*16;
-			size_t per_warp = P.fm_stride*4 + P.edge_stride*16 + P.rows_stride*8 + P.rowcnt_stride;
+			P.rows_stride = (size_t) ctx->plan_rmax[C]*MB_CAP;
+			P.rowcnt_stride = ((size_t) ctx->plan_rmax[C] + 31)/16*16;
+			size_t per_warp = P.fm_stride*4 + P.edge_stride*16 + P.rows_stride*8 + P.rowcnt_stride + MB_CHAIN_BUF*4;
 			if (free_b == 0)
 				cudaMemGetInfo(&free_b, &total_b);
-			const size_t have = free_b + ctx->d_fm[C].cap + ctx->d_edge[C].cap + ctx->d_rows[C].cap + ctx->d_rowcnt[C].cap;
+			const size_t held = ctx->d_fm[C].cap + ctx->d_edge[C].cap + ctx->d_rows[C].cap + ctx->d_rowcnt[C].cap
+			  + ctx->d_chainbuf[C].cap;
+			const size_t have = free_b + held;
 			size_t use_warps = nwarps;
 			if (per_warp*use_warps > have*8/10)
 				use_warps = std::max<size_t>(MB_WARPS_PER_BLOCK, (have*8/10/per_warp)/MB_WARPS_PER_BLOCK*MB_WARPS_PER_BLOCK);
 			nblocks = (uint32_t)(use_warps/MB_WARPS_PER_BLOCK);
-			const size_t cap_before = ctx->d_fm[C].cap + ctx->d_edge[C].cap + ctx->d_rows[C].cap + ctx->d_rowcnt[C].cap;
 			ENSURE(ctx->d_fm[C], P.fm_stride*4*use_warps);
 			ENSURE(ctx->d_edge[C], P.edge_stride*16*use_warps);
 			ENSURE(ctx->d_rows[C], P.rows_stride*8*use_warps);
 			ENSURE(ctx->d_rowcnt[C], P.rowcnt_stride*use_warps);
-			if (ctx->d_fm[C].cap + ctx->d_edge[C].cap + ctx->d_rows[C].cap + ctx->d_rowcnt[C].cap != cap_before)
+			ENSURE(ctx->d_chainbuf[C], (size_t) MB_CHAIN_BUF*4*use_warps);
+			if (ctx->d_fm[C].cap + ctx->d_edge[C].cap + ctx->d_rows[C].cap + ctx->d_rowcnt[C].cap + ctx->d_chainbuf[C].cap != held)
 				free_b = 0;                        // something was (re)allocated: ask again for the next size class
 			P.h = ctx->hmm;
 			P.matchT = (const float *)(mega ? ctx->d_megaT.p : ctx->d_matchT.p);
@@ -590,13 +632,15 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 			P.seqlen = (const uint32_t *) ctx->d_seqlen.p;
 			P.px = (const uint32_t *) ctx->d_px.p;
 			P.py = (const uint32_t *) ctx->d_py.p;
-			P.order = (const uint32_t *) ctx->d_order.p + bin_start[C];
-			P.nwork = (uint32_t) b.size();
+			P.order = (const uint32_t *) ctx->d_order.p;
+			P.chain = (const uint32_t *) ctx->d_chain.p + bin_start[C];
+			P.nwork = nchains;
 			P.counter = (uint32_t *)((char *) ctx->d_cursor.p + 16) + C;
 			P.fm = (float *) ctx->d_fm[C].p;
 			P.edge = (float4 *) ctx->d_edge[C].p;
 			P.rows = (mb200_entry *) ctx->d_rows[C].p;
 			P.rowcnt = (uint8_t *) ctx->d_rowcnt[C].p;
+			P.chainbuf = (uint32_t *) ctx->d_chainbuf[C].p;
 			P.rowoff = (uint32_t *) ctx->d_rowoff.p;
 			P.rowbase = (const uint64_t *) ctx->d_rowbase.p;
 			P.entries = (mb200_entry *) ctx->d_entries.p;

@@ -56,7 +56,7 @@ struct mb200_ctx
 	std::vector<uint32_t> h_nnz;
 	std::vector<uint64_t> h_entbase;
 	bool h_index_valid = false;
-	DevBuf d_px, d_py, d_order;
+	DevBuf d_px, d_py, d_order, d_chain;    // d_order: pairs chain after chain; d_chain: offsets of the chains in it
 	DevBuf d_rowoff, d_rowbase, d_entries, d_cursor, d_entbase, d_nnz, d_ea;     // d_cursor: control block, see prepare_plan
 	DevBuf d_entries2;                // second value buffer for the Jacobi update
 	DevBuf d_pack_off, d_pack_ent;    // packed image for exchange/export
@@ -82,11 +82,13 @@ struct mb200_ctx
 	bool plan_valid = false, plan_is_allpairs = false;
 	int plan_force_c = 0;
 	uint64_t plan_cells = 0, plan_est_entries = 0, last_used_entries = 0;
-	std::vector<std::vector<uint32_t>> plan_bins;
-	std::vector<uint32_t> plan_bin_start, plan_lxmax, plan_lymax;
+	std::vector<std::vector<uint32_t>> plan_bins;                 // pairs per size class
+	std::vector<uint32_t> plan_bin_start, plan_lxmax, plan_lymax;  // bin_start: first chain of each size class
+	std::vector<uint64_t> plan_fmax, plan_rmax;                    // largest chain: Forward rows (sum of LX+2), rows (sum of LX)
 
 	// per-warp scratch of the posterior kernel
 	DevBuf d_fm[MB_MAX_C + 1], d_edge[MB_MAX_C + 1], d_rows[MB_MAX_C + 1], d_rowcnt[MB_MAX_C + 1];   // per bin
+	DevBuf d_chainbuf[MB_MAX_C + 1];
 	static constexpr int kStreams = 4;          // column-width bins run concurrently to overlap their tails
 	cudaStream_t aux[kStreams] = {};
 	cudaEvent_t aux_done[kStreams] = {};

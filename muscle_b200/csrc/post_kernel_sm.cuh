@@ -6,8 +6,9 @@
 // (calcposteriorflat.cpp:4-27), MySparseMx::FromPost (mysparsemx.cpp:115-152) and CalcAlnScoreFlat
 // (calcalnscoreflat.cpp:4-32) of the reference.
 //
-// Mapping.  One warp owns one pair at a time (persistent warps pull pairs, longest first, from an
-// atomic cursor).  Lane l owns C consecutive DP columns of Y (C = ceil(LY/32) capped at the size
+// Mapping.  One warp owns one chain of pairs that share Y at a time (persistent warps pull chains,
+// longest first, from an atomic cursor; the wavefront fills and drains once per chain, see Forward
+// and Backward below).  Lane l owns C consecutive DP columns of Y (C = ceil(LY/32) capped at the size
 // class CM, a compile-time parameter); a warp therefore covers a strip of 32*C columns and longer Y
 // are processed strip after strip with the strip-edge column handed over through a small per-warp
 // buffer.  Rows of X are swept in anti-diagonal (wavefront) order: at step t lane l works on row t-l,
@@ -119,6 +120,9 @@ k_posterior_sm(const PostParams P)
 	float4      *edge1  = edge0 + (P.lxmax + 2);
 	mb200_entry *rows   = P.rows + (size_t) gwarp*P.rows_stride;
 	uint8_t     *rowcnt = P.rowcnt + (size_t) gwarp*P.rowcnt_stride;
+	uint32_t    *ckept  = P.chainbuf + (size_t) gwarp*MB_CHAIN_BUF;      // [pair of the chain][lane]
+	float       *ctotal = reinterpret_cast<float *>(ckept + MB_CHAIN_MAX*32);   // [pair of the chain]
+	float       *cfin   = ctotal + MB_CHAIN_MAX;                               // [pair of the chain][5]: cell (LX,LY)
 
 	for (;;)
 		{
@@ -128,29 +132,46 @@ k_posterior_sm(const PostParams P)
 		w = __shfl_sync(MB_FULL, w, 0);
 		if (w >= P.nwork)
 			break;
-		const uint32_t pair = P.order[w];
-		const uint32_t sx = P.px[pair], sy = P.py[pair];
-		const int LX = (int) P.seqlen[sx], LY = (int) P.seqlen[sy];
-		const uint8_t *Xc = P.codes + P.seqoff[sx];
+		// the work unit is a chain: P.order[chain[w] .. chain[w+1]) are pairs with the same Y, in store order
+		const uint32_t *cpairs = P.order + P.chain[w];
+		const int nch = (int)(P.chain[w + 1] - P.chain[w]);
+		const uint32_t sy = P.py[cpairs[0]];
+		const int LY = (int) P.seqlen[sy];
 		const uint8_t *Yc = P.codes + P.seqoff[sy];
-		// MEGA: 8 letter bytes and one insert emission per position
-		const uint2 *Xl = reinterpret_cast<const uint2 *>(P.codes) + P.seqoff[sx];
-		const uint2 *Yl = reinterpret_cast<const uint2 *>(P.codes) + P.seqoff[sy];
-		const float *Xi = P.insT + P.seqoff[sx];
-		const float *Yi = P.insT + P.seqoff[sy];
-		(void) Xc; (void) Yc; (void) Xl; (void) Yl; (void) Xi; (void) Yi;
-		const int C = min(min(CM, (int) P.cmax), (LY + 31) >> 5);   // columns per lane for this pair
+		const uint2 *Yl = reinterpret_cast<const uint2 *>(P.codes) + P.seqoff[sy];   // MEGA: 8 letter bytes per position
+		const float *Yi = P.insT + P.seqoff[sy];                                     // MEGA: insert emission per position
+		(void) Yc; (void) Yl; (void) Yi;
+		// per-lane pair cursor: the X side of pair k of the chain (loaded once per lane per pair)
+		int LX;
+		const uint8_t *Xc;
+		const uint2 *Xl;
+		const float *Xi;
+		auto load_x = [&](int k)
+			{
+			const uint32_t sx = P.px[cpairs[k]];
+			LX = (int) P.seqlen[sx];
+			Xc = P.codes + P.seqoff[sx];
+			Xl = reinterpret_cast<const uint2 *>(P.codes) + P.seqoff[sx];
+			Xi = P.insT + P.seqoff[sx];
+			};
+		const int sumLX = __reduce_add_sync(MB_FULL, lane < nch ? P.seqlen[P.px[cpairs[lane]]] : 0u);
+		const int C = min(min(CM, (int) P.cmax), (LY + 31) >> 5);   // columns per lane for this chain
 		const int W = 32*C;
-		const int nstrips = (LY + W - 1)/W;
+		const int nstrips = (LY + W - 1)/W;                 // > 1 only for a chain of one pair
 		const int lastj0 = (nstrips - 1)*W;
 		const int lcl = (LY - 1 - lastj0)/C;              // lane / local column of DP column LY
 		const int clast = (LY - 1 - lastj0) - lcl*C;
 
-		for (int k = lane; k < LX; k += 32)
+		for (int k = lane; k < sumLX; k += 32)
 			rowcnt[k] = 0;
+		for (int k = 0; k < nch; ++k)
+			ckept[k*32 + lane] = 0;
 
 		// ============================ Forward ============================
-		float fin0 = Z, fin1 = Z, fin2 = Z, fin3 = Z, fin4 = Z;
+		// Lane l steps through the chain's pairs one after the other: rows 0..LX of a pair, then one
+		// separator step that resets the lane's state records to LOG_ZERO and passes LOG_ZERO on, so
+		// that row 0 of the next pair sees exactly the border of a fresh pair.  Pair k starts at chain
+		// step Fk + l, Fk = sum over earlier pairs of (LX + 2).
 		for (int strip = 0; strip < nstrips; ++strip)
 			{
 			const int j0 = strip*W;
@@ -181,13 +202,15 @@ k_posterior_sm(const PostParams P)
 			float outM = Z, outAIY = Z, outAJY = Z, outS = Z;
 			float dprev = Z;
 			float bIX = Z, bJX = Z;
-			const int nsteps = LX + nl;
+			const int nsteps = sumLX + 2*nch - 2 + nl;
 			int xcPref = h.pad;
 			uint2 xlPref = make_uint2(0u, 0u);
 			float exPref = 0.0f;
+			int kp = 0, r0 = lane;                // the lane's pair and the step of its row 0
+			load_x(0);
 			for (int t = 0; t < nsteps; ++t)
 				{
-				const int i = t - lane;
+				const int i = t - r0;
 				const int xc = xcPref;
 				const uint2 xl = xlPref;
 				const float exm = exPref;
@@ -279,32 +302,52 @@ MB_UNROLL(MB_SM_UNROLL)
 						}
 					if (last && i == LX && lane == lcl)    // cell (LX,LY) is the lane's last
 						{
-						fin0 = lm; fin1 = ix; fin2 = iy; fin3 = jx; fin4 = jy;
+						float *f = cfin + 5*kp;
+						f[0] = lm; f[1] = ix; f[2] = iy; f[3] = jx; f[4] = jy;
 						}
 					outM = lm; outAIY = laiy; outAJY = lajy; outS = sLast;
 					if (lane == 31 && !last)
 						edgeOut[i] = make_float4(outM, outAIY, outAJY, outS);
 					}
+				else if (i == LX + 1 && lane < nl)        // separator, then the next pair of the chain
+					{
+#pragma unroll 1
+					for (int c = 0; c < C; ++c)
+						st[c*32 + lane] = make_float4(Z, Z, Z, Z);
+					outM = Z; outAIY = Z; outAJY = Z; outS = Z;
+					dprev = Z;
+					if (++kp < nch)
+						{
+						load_x(kp);
+						r0 = t + 1;
+						}
+					else
+						r0 = 1 << 30;                 // done: idle for the rest of the strip
+					}
 				}
 			__syncwarp();
 			}
 
-		// ============================ total probability ============================
-		fin0 = __shfl_sync(MB_FULL, fin0, lcl);
-		fin1 = __shfl_sync(MB_FULL, fin1, lcl);
-		fin2 = __shfl_sync(MB_FULL, fin2, lcl);
-		fin3 = __shfl_sync(MB_FULL, fin3, lcl);
-		fin4 = __shfl_sync(MB_FULL, fin4, lcl);
-		float total = Z;
-		total = la(total, ADD(fin0, h.tSM));
-		total = la(total, ADD(fin1, h.tSI));
-		total = la(total, ADD(fin2, h.tSI));
-		total = la(total, ADD(fin3, h.tSJ));
-		total = la(total, ADD(fin4, h.tSJ));
-		if (DUMP && lane == 0)
-			*P.dbg_total = total;
+		// ============================ total probability, lane k for pair k ============================
+		if (lane < nch)
+			{
+			const float *f = cfin + 5*lane;
+			float total = Z;
+			total = la(total, ADD(f[0], h.tSM));
+			total = la(total, ADD(f[1], h.tSI));
+			total = la(total, ADD(f[2], h.tSI));
+			total = la(total, ADD(f[3], h.tSJ));
+			total = la(total, ADD(f[4], h.tSJ));
+			ctotal[lane] = total;
+			if (DUMP)
+				*P.dbg_total = total;
+			}
+		__syncwarp();
 
 		// ============================ Backward + posterior ============================
+		// The chain's pairs last to first, rows LX..1 of a pair and then a separator step; pair k starts
+		// at chain step (sum over later pairs of (LX + 1)) + nl-1-l.  ckept[k][l] counts the lane's
+		// kept entries up to the end of pair k, so that each pair's count is a difference.
 		uint32_t kept = 0;
 		bool overflow = false;
 		for (int strip = nstrips - 1; strip >= 0; --strip)
@@ -336,13 +379,18 @@ MB_UNROLL(MB_SM_UNROLL)
 				}
 			float outM = Z, outIY = Z, outJY = Z;
 			float dprev = Z;
-			const int nsteps = LX + nl - 1;
+			const int nsteps = sumLX + nch - 2 + nl;
 			int xcPref = h.pad;
 			uint2 xlPref = make_uint2(0u, 0u);
 			float exPref = 0.0f;
+			int kp = nch - 1, u0 = nl - 1 - lane;   // the lane's pair and the step of its row LX
+			load_x(nch - 1);
+			int fk = sumLX - LX + 2*(nch - 1);      // chain Forward step of the pair's row 0, less the lane
+			int rk = sumLX - LX;                  // chain row of the pair's row 1 in rows / rowcnt
+			float total = ctotal[nch - 1];
 			for (int u = 0; u < nsteps; ++u)
 				{
-				const int i = LX - u + (nl - 1 - lane);
+				const int i = LX - u + u0;
 				const int xc = xcPref;
 				const uint2 xl = xlPref;
 				const float exm = exPref;
@@ -381,10 +429,10 @@ MB_UNROLL(MB_SM_UNROLL)
 						for (int f = 0; f < 8; ++f)
 							xb[f] = P.mega_base[f] + ((f < 4 ? (xl.x >> (8*f)) : (xl.y >> (8*(f - 4)))) & 255u)*P.mega_alpha[f];
 						}
-					uint32_t cnt = rowcnt[i - 1];
+					uint32_t cnt = rowcnt[rk + i - 1];
 					const uint32_t cnt0 = cnt;
-					mb200_entry *row = rows + (size_t)(i - 1)*MB_CAP;
-					const int t = i + lane;
+					mb200_entry *row = rows + (size_t)(rk + i - 1)*MB_CAP;
+					const int t = fk + i + lane;
 					const int col0 = j0 + lane*C;
 					float mdiag = dprev;
 					dprev = Rm;
@@ -464,144 +512,174 @@ MB_UNROLL(MB_SM_UNROLL)
 					if (lane == 0 && strip > 0)
 						edgeOut[i] = make_float4(outM, outIY, outJY, 0.0f);
 					if (cnt != cnt0)
-						rowcnt[i - 1] = (uint8_t) min(cnt, (uint32_t) MB_CAP);
+						rowcnt[rk + i - 1] = (uint8_t) min(cnt, (uint32_t) MB_CAP);
+					}
+				else if (i == 0 && lane < nl)         // separator, then the previous pair of the chain
+					{
+#pragma unroll 1
+					for (int c = 0; c < C; ++c)
+						st[c*32 + lane] = make_float4(Z, Z, Z, Z);
+					outM = Z; outIY = Z; outJY = Z;
+					dprev = Z;
+					ckept[kp*32 + lane] = kept;
+					if (kp > 0)
+						{
+						load_x(--kp);
+						u0 = u + 1;
+						fk -= LX + 2;
+						rk -= LX;
+						total = ctotal[kp];
+						}
+					else
+						u0 = -(1 << 30);              // done: idle for the rest of the strip
 					}
 				__syncwarp();
 				}
 			}
-
-		// ============================ compaction + expected accuracy ============================
+		ckept[lane] = kept;                       // the end of pair 0 (its separator may lie past the last step)
 		overflow = __any_sync(MB_FULL, overflow);
-		for (int o = 16; o > 0; o >>= 1)
-			kept += __shfl_xor_sync(MB_FULL, kept, o);
-		unsigned long long base = 0;
-		if (lane == 0)
-			base = atomicAdd(P.ent_cursor, (unsigned long long) kept);
-		base = __shfl_sync(MB_FULL, base, 0);
-		const bool fits = (base + kept <= P.ent_cap);
-		if (lane == 0)
-			{
-			if (overflow)
-				atomicCAS(P.err, 0, MB200_EOVERFLOW);
-			if (!fits)
-				atomicCAS(P.err, 0, MB200_ENOMEM);
-			P.entbase[pair] = base;
-			P.nnz[pair] = kept;
-			}
-		uint32_t *rowoff = P.rowoff + P.rowbase[pair];
-		mb200_entry *out = P.entries + base;
-
-		float eaScore = 0.0f;
-		{
-		// the warp's state area, reused as three plain float arrays of CM*32
-		float *old = wbase;                 // [c][lane]
-		float *rowbuf = wbase + CM*32;      // column-linear: [lane*C + c]
-		float *pre = wbase + 2*CM*32;       // [c][lane]
-		float *eIn = reinterpret_cast<float *>(edge0);
-		float *eOut = reinterpret_cast<float *>(edge1);
-		uint32_t written = 0;
-		for (int strip = 0; strip < nstrips; ++strip)
-			{
-			const int j0 = strip*W;
-			for (int c = 0; c < C; ++c)
-				{
-				old[c*32 + lane] = 0.0f;
-				rowbuf[c*32 + lane] = 0.0f;
-				}
-			__syncwarp();
-			for (int i = 1; i <= LX; ++i)
-				{
-				const uint32_t cnt = rowcnt[i - 1];
-				const mb200_entry *row = rows + (size_t)(i - 1)*MB_CAP;
-				if (strip == 0 && lane == 0)
-					rowoff[i - 1] = written;
-				for (uint32_t e0 = 0; e0 < cnt; e0 += 32)
-					{
-					const int idx = (int) cnt - 1 - (int)(e0 + lane);
-					mb200_entry ent; ent.p = 0.0f; ent.col = 0;
-					if (idx >= 0)
-						ent = row[idx];
-					const int lc = (int) ent.col - j0;
-					if (idx >= 0 && lc >= 0 && lc < W)
-						rowbuf[lc] = ent.p;
-					if (strip == 0)
-						{
-						const bool keep = idx >= 0 && ent.p >= 0.01f;          // mysparsemx.cpp:139-141
-						const uint32_t b = __ballot_sync(MB_FULL, keep);
-						if (keep && fits)
-							out[written + __popc(b & ((1u << lane) - 1u))] = ent;
-						written += __popc(b);
-						}
-					}
-				__syncwarp();
-				// calcalnscoreflat.cpp:13-29 as a prefix-max over the row
-				float leftOld = 0.0f, incoming = 0.0f;
-				if (lane == 0)
-					{
-					leftOld = strip == 0 ? 0.0f : eIn[i - 1];
-					incoming = strip == 0 ? 0.0f : eIn[i];
-					}
-				else
-					leftOld = old[(C - 1)*32 + lane - 1];
-				float run = 0.0f, prevOld = leftOld;
-				for (int c = 0; c < C; ++c)
-					{
-					const float o = old[c*32 + lane];
-					const float b = ADD(prevOld, rowbuf[lane*C + c]);
-					float v = fmaxf(o, b);
-					v = c == 0 ? v : fmaxf(v, run);
-					run = v;
-					pre[c*32 + lane] = v;
-					prevOld = o;
-					}
-				__syncwarp();
-				float scan = run;
-#pragma unroll
-				for (int o = 1; o < 32; o <<= 1)
-					{
-					const float n = __shfl_up_sync(MB_FULL, scan, o);
-					if (lane >= o)
-						scan = fmaxf(scan, n);
-					}
-				float excl = __shfl_up_sync(MB_FULL, scan, 1);
-				const float inc0 = __shfl_sync(MB_FULL, incoming, 0);
-				excl = lane == 0 ? inc0 : fmaxf(excl, inc0);
-				float lastNew = 0.0f;
-				for (int c = 0; c < C; ++c)
-					{
-					lastNew = fmaxf(pre[c*32 + lane], excl);
-					old[c*32 + lane] = lastNew;
-					}
-				if (lane == 31 && strip + 1 < nstrips)
-					eOut[i] = lastNew;
-				__syncwarp();
-				for (uint32_t e0 = 0; e0 < cnt; e0 += 32)
-					{
-					const int idx = (int) cnt - 1 - (int)(e0 + lane);
-					if (idx >= 0)
-						{
-						const int lc = (int) row[idx].col - j0;
-						if (lc >= 0 && lc < W)
-							rowbuf[lc] = 0.0f;
-						}
-					}
-				__syncwarp();
-				}
-			if (strip == 0 && lane == 0)
-				rowoff[LX] = written;
-			if (lane == 31 && strip + 1 < nstrips)
-				eOut[0] = 0.0f;
-			if (strip == nstrips - 1)
-				{
-				const int q = LY - 1 - j0;          // column-local index of DP column LY
-				eaScore = old[(q % C)*32 + q/C];
-				}
-			__syncwarp();
-			float *tmp = eIn; eIn = eOut; eOut = tmp;
-			}
-		}
-		if (lane == 0)
-			P.ea[pair] = __fdiv_rn(eaScore, (float) min(LX, LY));     // calcposteriorflat.cpp:89
+		if (lane == 0 && overflow)
+			atomicCAS(P.err, 0, MB200_EOVERFLOW);
 		__syncwarp();
+
+		// ============================ compaction + expected accuracy, pair by pair ============================
+		int rk = 0;
+		for (int k = 0; k < nch; rk += LX, ++k)
+			{
+			const uint32_t pair = cpairs[k];
+			LX = (int) P.seqlen[P.px[pair]];
+			uint32_t kept = ckept[k*32 + lane] - (k + 1 < nch ? ckept[(k + 1)*32 + lane] : 0u);
+			for (int o = 16; o > 0; o >>= 1)
+				kept += __shfl_xor_sync(MB_FULL, kept, o);
+			unsigned long long base = 0;
+			if (lane == 0)
+				base = atomicAdd(P.ent_cursor, (unsigned long long) kept);
+			base = __shfl_sync(MB_FULL, base, 0);
+			const bool fits = (base + kept <= P.ent_cap);
+			if (lane == 0)
+				{
+				if (!fits)
+					atomicCAS(P.err, 0, MB200_ENOMEM);
+				P.entbase[pair] = base;
+				P.nnz[pair] = kept;
+				}
+			const mb200_entry *prow = rows + (size_t) rk*MB_CAP;
+			const uint8_t *pcnt = rowcnt + rk;
+			uint32_t *rowoff = P.rowoff + P.rowbase[pair];
+			mb200_entry *out = P.entries + base;
+
+			float eaScore = 0.0f;
+			{
+			// the warp's state area, reused as three plain float arrays of CM*32
+			float *old = wbase;                 // [c][lane]
+			float *rowbuf = wbase + CM*32;      // column-linear: [lane*C + c]
+			float *pre = wbase + 2*CM*32;       // [c][lane]
+			float *eIn = reinterpret_cast<float *>(edge0);
+			float *eOut = reinterpret_cast<float *>(edge1);
+			uint32_t written = 0;
+			for (int strip = 0; strip < nstrips; ++strip)
+				{
+				const int j0 = strip*W;
+				for (int c = 0; c < C; ++c)
+					{
+					old[c*32 + lane] = 0.0f;
+					rowbuf[c*32 + lane] = 0.0f;
+					}
+				__syncwarp();
+				for (int i = 1; i <= LX; ++i)
+					{
+					const uint32_t cnt = pcnt[i - 1];
+					const mb200_entry *row = prow + (size_t)(i - 1)*MB_CAP;
+					if (strip == 0 && lane == 0)
+						rowoff[i - 1] = written;
+					for (uint32_t e0 = 0; e0 < cnt; e0 += 32)
+						{
+						const int idx = (int) cnt - 1 - (int)(e0 + lane);
+						mb200_entry ent; ent.p = 0.0f; ent.col = 0;
+						if (idx >= 0)
+							ent = row[idx];
+						const int lc = (int) ent.col - j0;
+						if (idx >= 0 && lc >= 0 && lc < W)
+							rowbuf[lc] = ent.p;
+						if (strip == 0)
+							{
+							const bool keep = idx >= 0 && ent.p >= 0.01f;          // mysparsemx.cpp:139-141
+							const uint32_t b = __ballot_sync(MB_FULL, keep);
+							if (keep && fits)
+								out[written + __popc(b & ((1u << lane) - 1u))] = ent;
+							written += __popc(b);
+							}
+						}
+					__syncwarp();
+					// calcalnscoreflat.cpp:13-29 as a prefix-max over the row
+					float leftOld = 0.0f, incoming = 0.0f;
+					if (lane == 0)
+						{
+						leftOld = strip == 0 ? 0.0f : eIn[i - 1];
+						incoming = strip == 0 ? 0.0f : eIn[i];
+						}
+					else
+						leftOld = old[(C - 1)*32 + lane - 1];
+					float run = 0.0f, prevOld = leftOld;
+					for (int c = 0; c < C; ++c)
+						{
+						const float o = old[c*32 + lane];
+						const float b = ADD(prevOld, rowbuf[lane*C + c]);
+						float v = fmaxf(o, b);
+						v = c == 0 ? v : fmaxf(v, run);
+						run = v;
+						pre[c*32 + lane] = v;
+						prevOld = o;
+						}
+					__syncwarp();
+					float scan = run;
+#pragma unroll
+					for (int o = 1; o < 32; o <<= 1)
+						{
+						const float n = __shfl_up_sync(MB_FULL, scan, o);
+						if (lane >= o)
+							scan = fmaxf(scan, n);
+						}
+					float excl = __shfl_up_sync(MB_FULL, scan, 1);
+					const float inc0 = __shfl_sync(MB_FULL, incoming, 0);
+					excl = lane == 0 ? inc0 : fmaxf(excl, inc0);
+					float lastNew = 0.0f;
+					for (int c = 0; c < C; ++c)
+						{
+						lastNew = fmaxf(pre[c*32 + lane], excl);
+						old[c*32 + lane] = lastNew;
+						}
+					if (lane == 31 && strip + 1 < nstrips)
+						eOut[i] = lastNew;
+					__syncwarp();
+					for (uint32_t e0 = 0; e0 < cnt; e0 += 32)
+						{
+						const int idx = (int) cnt - 1 - (int)(e0 + lane);
+						if (idx >= 0)
+							{
+							const int lc = (int) row[idx].col - j0;
+							if (lc >= 0 && lc < W)
+								rowbuf[lc] = 0.0f;
+							}
+						}
+					__syncwarp();
+					}
+				if (strip == 0 && lane == 0)
+					rowoff[LX] = written;
+				if (lane == 31 && strip + 1 < nstrips)
+					eOut[0] = 0.0f;
+				if (strip == nstrips - 1)
+					{
+					const int q = LY - 1 - j0;          // column-local index of DP column LY
+					eaScore = old[(q % C)*32 + q/C];
+					}
+				__syncwarp();
+				float *tmp = eIn; eIn = eOut; eOut = tmp;
+				}
+			}
+			if (lane == 0)
+				P.ea[pair] = __fdiv_rn(eaScore, (float) min(LX, LY));     // calcposteriorflat.cpp:89
+			__syncwarp();
+			}
 		}
 	}
