@@ -223,6 +223,21 @@ int mb200_debug_force_c(mb200_ctx *ctx, int c);
 /* expected entries per posterior row used to size the entry pool (default 12; the pool is re-sized
  * with the exact count and the stage re-run if it was too small) */
 int mb200_set_nnz_per_row_cap(mb200_ctx *ctx, uint32_t cap);
+/* The work plan of the last posterior call, as the kernel reads it.  A chain is a run of pairs that
+ * share Y and that one warp computes back to back; chain c is order[chain[c] .. chain[c+1]) (store
+ * pair ids).  *npairs and *nchains are always set; order[npairs], chain[nchains+1], bin_start[18]
+ * (bin_start[C] = first chain of the pairs run at C columns per lane, C = 1..16; bin_start[17] =
+ * nchains) and limits[2] (the most Forward rows, sum of LX+2, and the most pairs in one chain) are
+ * filled when not NULL, so a first call with NULL arrays returns the counts. */
+int mb200_debug_plan(mb200_ctx *ctx, uint32_t *npairs, uint32_t *nchains, uint32_t *order, uint32_t *chain,
+                     uint32_t *bin_start, uint32_t *limits);
+/* mb200_calc_post_dense for store pair `which` of a pair list: runs the whole list as
+ * mb200_posteriors does (same chains, the store and EA are filled too) and copies out the dense
+ * results of that one pair, at whatever position of its chain it runs.  Honours
+ * mb200_debug_force_c.  mb200_calc_post_dense(x, y) is the one-pair case. */
+int mb200_calc_post_dense_pair(mb200_ctx *ctx, uint32_t npairs, const uint32_t *pair_x, const uint32_t *pair_y,
+                               uint32_t which, float *post_out, float *fwd_m_out, float *bwd_m_out,
+                               float *total_out);
 
 /* ---- several GPUs from one process (SURVEY.md section 8b: "mb200_create(ndev, ...)") -------- */
 /* A group is ndev single-device contexts plus the two exchange steps of the path (section 8e).

@@ -174,6 +174,7 @@ struct PostParams
 	uint32_t       *nnz;            // per store pair
 	float          *ea;             // per store pair
 	int            *err;            // sticky error code
-	// optional dense dumps for one pair (parity surface, mb200_calc_post_dense)
+	// optional dense dumps for one pair (parity surface, mb200_calc_post_dense_pair)
 	float *dbg_fwd, *dbg_bwd, *dbg_post, *dbg_total;
+	uint32_t dbg_pair;              // the store pair they are written for
 	};

@@ -575,7 +575,7 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 				memset(ctx->occ_cache, 0, sizeof ctx->occ_cache);
 				ctx->occ_cache_k = tsize*2 + (mega ? 1 : 0);
 				}
-			if (dump)          // one pair, another instantiation: not cached
+			if (dump)          // another instantiation: not cached
 				mb_post_sm_dispatch(mega, dump, CM, 1, dim3(), smem, ks, nullptr, &occ);
 			else
 				{
@@ -653,6 +653,7 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 			if (dbg)
 				{
 				P.dbg_fwd = dbg->fwd; P.dbg_bwd = dbg->bwd; P.dbg_post = dbg->post; P.dbg_total = dbg->total;
+				P.dbg_pair = dbg->pair;
 				}
 			P.cmax = (uint32_t) C;
 			mb_post_sm_dispatch(mega, dump, CM, 0, dim3(nblocks), smem, ks, &P, nullptr);
@@ -781,18 +782,19 @@ int mb200_posteriors_allpairs(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi, floa
 	return rc;
 	}
 
-int mb200_calc_post_dense(mb200_ctx *ctx, uint32_t x, uint32_t y, float *post_out, float *fwd_m_out,
-  float *bwd_m_out, float *total_out)
+int mb200_calc_post_dense_pair(mb200_ctx *ctx, uint32_t npairs, const uint32_t *pair_x, const uint32_t *pair_y,
+  uint32_t which, float *post_out, float *fwd_m_out, float *bwd_m_out, float *total_out)
 	{
-	if (!ctx || !post_out || x >= ctx->nseq || y >= ctx->nseq)
-		return mb_fail(ctx, MB200_EINVAL, "mb200_calc_post_dense: bad argument");
+	if (!ctx || !post_out || !pair_x || !pair_y || which >= npairs || pair_x[which] >= ctx->nseq
+	  || pair_y[which] >= ctx->nseq)
+		return mb_fail(ctx, MB200_EINVAL, "mb200_calc_post_dense_pair: bad argument");
 	cudaSetDevice(ctx->device);
-	const size_t n = (size_t) ctx->h_len[x]*ctx->h_len[y];
+	const size_t n = (size_t) ctx->h_len[pair_x[which]]*ctx->h_len[pair_y[which]];
 	ENSURE(ctx->d_dbg, (3*n + 4)*sizeof(float));
 	float *base = (float *) ctx->d_dbg.p;
-	PostDebug dbg = { base, base + n, base + 2*n, base + 3*n };
-	ctx->h_px.assign(1, x);
-	ctx->h_py.assign(1, y);
+	PostDebug dbg = { base, base + n, base + 2*n, base + 3*n, which };
+	ctx->h_px.assign(pair_x, pair_x + npairs);
+	ctx->h_py.assign(pair_y, pair_y + npairs);
 	ctx->store_allpairs = false;
 	ctx->ea_allpairs = false;
 	ctx->store_valid = false;
@@ -808,6 +810,38 @@ int mb200_calc_post_dense(mb200_ctx *ctx, uint32_t x, uint32_t y, float *post_ou
 		CU(cudaMemcpy(bwd_m_out, dbg.bwd, n*sizeof(float), cudaMemcpyDeviceToHost));
 	if (total_out)
 		CU(cudaMemcpy(total_out, dbg.total, sizeof(float), cudaMemcpyDeviceToHost));
+	return MB200_OK;
+	}
+
+int mb200_calc_post_dense(mb200_ctx *ctx, uint32_t x, uint32_t y, float *post_out, float *fwd_m_out,
+  float *bwd_m_out, float *total_out)
+	{
+	return mb200_calc_post_dense_pair(ctx, 1, &x, &y, 0, post_out, fwd_m_out, bwd_m_out, total_out);
+	}
+
+// test hook: the plan of the last posterior call, as the kernel reads it
+int mb200_debug_plan(mb200_ctx *ctx, uint32_t *npairs, uint32_t *nchains, uint32_t *order, uint32_t *chain,
+  uint32_t *bin_start, uint32_t *limits)
+	{
+	if (!ctx || !npairs || !nchains)
+		return mb_fail(ctx, MB200_EINVAL, "mb200_debug_plan: bad argument");
+	if (!ctx->plan_valid)
+		return mb_fail(ctx, MB200_EINVAL, "mb200_debug_plan: no plan (run a posterior stage first)");
+	cudaSetDevice(ctx->device);
+	const uint32_t np = (uint32_t) ctx->h_px.size(), nc = ctx->plan_bin_start[MB_MAX_C + 1];
+	*npairs = np;
+	*nchains = nc;
+	if (order)
+		CU(cudaMemcpy(order, ctx->d_order.p, np*sizeof(uint32_t), cudaMemcpyDeviceToHost));
+	if (chain)
+		CU(cudaMemcpy(chain, ctx->d_chain.p, (nc + 1)*sizeof(uint32_t), cudaMemcpyDeviceToHost));
+	if (bin_start)
+		memcpy(bin_start, ctx->plan_bin_start.data(), (MB_MAX_C + 2)*sizeof(uint32_t));
+	if (limits)
+		{
+		limits[0] = (uint32_t) kChainRows;
+		limits[1] = MB_CHAIN_MAX;
+		}
 	return MB200_OK;
 	}
 

@@ -11,7 +11,7 @@ struct DevBuf
 	void release();
 	};
 
-struct PostDebug { float *fwd, *bwd, *post, *total; };
+struct PostDebug { float *fwd, *bwd, *post, *total; uint32_t pair; };
 
 struct mb200_ctx
 	{

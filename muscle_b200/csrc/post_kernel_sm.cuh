@@ -46,8 +46,9 @@
 // them in order -- and the insert emission is a per-position value precomputed the same way
 // (Mega::GetInsScore, mega.cpp:273-286).  Same recurrences, same kernel, one template flag.
 //
-// DUMP: the instantiation used by mb200_calc_post_dense also writes the dense Forward-M, Backward-M,
-// posterior and total of its pair; production launches carry no dump code.
+// DUMP: the instantiation used by mb200_calc_post_dense_pair runs the whole pair list with the same
+// chains and also writes the dense Forward-M, Backward-M, posterior and total of store pair
+// P.dbg_pair, wherever it sits in its chain; production launches carry no dump code.
 #pragma once
 #include "common.cuh"
 
@@ -275,7 +276,8 @@ k_posterior_sm(const PostParams P)
 					const uint2 *yp = ye + lane;
 					const uint32_t *y2p = y2 + lane;
 					float *dst = fms + (size_t) t*W + lane;
-					(void) y2p;
+					const bool dump = DUMP && i >= 1 && cpairs[kp] == P.dbg_pair;
+					(void) y2p; (void) dump;
 MB_UNROLL(MB_SM_UNROLL)
 					for (int c = 0; c < cn; ++c, sp += 32, yp += 32, y2p += 32, dst += 32)
 						{
@@ -297,7 +299,7 @@ MB_UNROLL(MB_SM_UNROLL)
 						lajy = ADD(jy, h.tJJ);
 						sLast = s;
 						*dst = m;
-						if (DUMP && i >= 1)
+						if (dump)
 							P.dbg_fwd[(size_t)(i - 1)*LY + j0 + lane*C + c] = m;
 						}
 					if (last && i == LX && lane == lcl)    // cell (LX,LY) is the lane's last
@@ -339,7 +341,7 @@ MB_UNROLL(MB_SM_UNROLL)
 			total = la(total, ADD(f[3], h.tSJ));
 			total = la(total, ADD(f[4], h.tSJ));
 			ctotal[lane] = total;
-			if (DUMP)
+			if (DUMP && cpairs[lane] == P.dbg_pair)
 				*P.dbg_total = total;
 			}
 		__syncwarp();
@@ -454,7 +456,7 @@ MB_UNROLL(MB_SM_UNROLL)
 							++cnt;
 							kept += (p >= 0.01f) ? 1u : 0u;
 							}
-						if (DUMP)
+						if (DUMP && cpairs[kp] == P.dbg_pair)
 							{
 							P.dbg_bwd[(size_t)(i - 1)*LY + col0 + c] = m;
 							P.dbg_post[(size_t)(i - 1)*LY + col0 + c] =

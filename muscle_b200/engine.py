@@ -18,7 +18,7 @@ EXPORTS = [
 	"mb200_export_pair", "mb200_export_all", "mb200_store_pack", "mb200_store_load_allpairs",
 	"mb200_store_values", "mb200_store_set_values", "mb200_consistency_iter", "mb200_align_pairs",
 	"mb200_align_groups", "mb200_calc_post_dense", "mb200_get_stats", "mb200_residue_classes",
-	"mb200_debug_force_c", "mb200_set_nnz_per_row_cap",
+	"mb200_debug_force_c", "mb200_set_nnz_per_row_cap", "mb200_debug_plan", "mb200_calc_post_dense_pair",
 	"mb200_store_exchange_begin", "mb200_store_exchange_commit", "mb200_store_entries_ptr", "mb200_store_values_changed",
 	"mb200_group_create", "mb200_group_destroy", "mb200_group_last_error", "mb200_group_size", "mb200_group_ctx",
 	"mb200_group_set_hmm", "mb200_group_set_seqs", "mb200_group_posteriors_allpairs", "mb200_group_consistency_iter",
@@ -198,17 +198,41 @@ class Engine:
 		return offs, ents
 
 	def calc_post_dense(self, x, y, force_c=0):
-		LX, LY = int(self.lens[x]), int(self.lens[y])
-		self.lib.mb200_debug_force_c(self.h, int(force_c))
+		return self.calc_post_dense_pair([x], [y], 0, force_c)
+
+	def calc_post_dense_pair(self, pair_x, pair_y, which, force_c=0):
+		"""dense (post, Forward-M, Backward-M, total) of store pair `which`, run inside the whole list"""
+		px = np.ascontiguousarray(pair_x, np.uint32)
+		py = np.ascontiguousarray(pair_y, np.uint32)
+		LX, LY = int(self.lens[px[which]]), int(self.lens[py[which]])
 		post = np.empty((LX, LY), np.float32)
 		fwd = np.empty((LX, LY), np.float32)
 		bwd = np.empty((LX, LY), np.float32)
 		tot = C.c_float()
-		self._ck(self.lib.mb200_calc_post_dense(self.h, C.c_uint32(x), C.c_uint32(y), _ptr(post), _ptr(fwd),
-		  _ptr(bwd), C.byref(tot)))
-		self.lib.mb200_debug_force_c(self.h, 0)
-		self._pairs = (np.array([x], np.uint32), np.array([y], np.uint32))
+		self._ck(self.lib.mb200_debug_force_c(self.h, int(force_c)))
+		try:
+			self._ck(self.lib.mb200_calc_post_dense_pair(self.h, C.c_uint32(len(px)), _ptr(px), _ptr(py),
+			  C.c_uint32(which), _ptr(post), _ptr(fwd), _ptr(bwd), C.byref(tot)))
+		finally:
+			self.lib.mb200_debug_force_c(self.h, 0)
+		self._pairs = (px, py)
 		return post, fwd, bwd, tot.value
+
+	def debug_plan(self):
+		"""the plan of the last posterior call: dict(order, chain, bin_start, chain_rows, chain_pairs)"""
+		npairs, nchains = C.c_uint32(), C.c_uint32()
+		self._ck(self.lib.mb200_debug_plan(self.h, C.byref(npairs), C.byref(nchains), None, None, None, None))
+		order = np.empty(npairs.value, np.uint32)
+		chain = np.empty(nchains.value + 1, np.uint32)
+		bin_start = np.empty(18, np.uint32)
+		limits = np.empty(2, np.uint32)
+		self._ck(self.lib.mb200_debug_plan(self.h, C.byref(npairs), C.byref(nchains), _ptr(order), _ptr(chain),
+		  _ptr(bin_start), _ptr(limits)))
+		return {"order": order, "chain": chain, "bin_start": bin_start, "chain_rows": int(limits[0]),
+		  "chain_pairs": int(limits[1])}
+
+	def set_nnz_per_row_cap(self, cap):
+		self._ck(self.lib.mb200_set_nnz_per_row_cap(self.h, C.c_uint32(cap)))
 
 	# ---- consistency
 	def consistency_iter(self, p_lo=0, p_hi=None):
