@@ -14,6 +14,8 @@
 #define MB_MAX_K 64                    // residue classes the smem tables can hold
 #define MB_CAP MB200_MAX_ROW_NNZ       // candidate entries per posterior row
 #define MB_WARPS_PER_BLOCK 4            // posterior kernel: warps (chains in flight) per CTA
+#define MB_SM_ARRAYS 5                  // posterior kernel: shared words per (column, lane): float4 state + class of Y
+#define MB_SM_ARRAYS_MEGA 7             // MEGA: float4 state + {letters 0..3, eY} + letters 4..7
 #define MB_CHAIN_MAX 32                 // posterior kernel: pairs in one chain (one per lane when the chain is read)
 #define MB_CHAIN_BUF (MB_CHAIN_MAX*38)  // words of per-warp chain scratch: kept counts [pair][lane], totals [pair], final cells [pair][5]
 
@@ -46,8 +48,11 @@ __constant__ float4 c_logexp1[4] =
 //    is found WITHOUT compares: k = ceil(2d) is formed in the mantissa of 2d + 1.5*2^23 by one
 //    FFMA with round-up, and k*16 added to a pre-biased base is the shared-memory address of a
 //    17-entry {c3,c2,c1,c0} table (k = 0..2 -> piece 0, 3..5 -> 1, 6..9 -> 2, 10..16 -> 3).  The gap is
-//    clamped to 7.75 before the index is formed, so the load is always inside the table; for d >= 7.5 the
-//    polynomial result is discarded by the final select.  A form with two compare/select pairs for
+//    clamped to 4.75 before the index is formed: every d > 4.5 then reads entry 10 (piece 3, as before;
+//    for d >= 7.5 the polynomial result is discarded by the final select).  The 32 lanes of a load so
+//    touch at most 11 entries, not 17; entries k and k+8 share banks, and the kernels that use this are
+//    bound by shared-memory wavefronts as much as by issue (clamping at 7.75 measured 1.5 % slower in
+//    k_posterior_sm, H100 80GB HBM3 at 400 W).  A form with two compare/select pairs for
 //    the piece takes 17 instructions per LOG_ADD, 8 of them on the half-rate ALU pipe; this form is
 //    14 instructions with 4 on the ALU pipe.
 //  The arithmetic (sub, three mul/add Horner steps with separate roundings, final add) is written
@@ -61,8 +66,8 @@ struct LogAdd
 		const float d = fabsf(__fsub_rn(x, y));
 		const float lo = fminf(x, y);
 		const float hi = fmaxf(x, y);
-		// the address stays inside the 17-entry table for any gap (entry 16 is never used for a result)
-		const float t = __fmaf_ru(fminf(d, 7.75f), 2.0f, 12582912.0f);
+		// the address stays inside the 17-entry table for any gap (entries 11..16 are no longer read)
+		const float t = __fmaf_ru(fminf(d, 4.75f), 2.0f, 12582912.0f);
 		const uint32_t addr = tab + (__float_as_uint(t) << 4);
 		float4 c;
 		asm("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(c.x), "=f"(c.y), "=f"(c.z), "=f"(c.w) : "r"(addr));

@@ -564,12 +564,13 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 			const bool mega = ctx->mega;
 			const bool dump = dbg != nullptr;
 			const int CM = mb_post_sm_class(C);      // == C unless the width is forced
-			const int tsize = mega ? (int) ctx->mega_tsize : ctx->hmm.K*ctx->hmm.KS;
+			// floats of the emission table in shared memory (plain mode: {match, ins} pairs, see k_posterior_sm)
+			const int tsize = mega ? (int) ctx->mega_tsize : 2*ctx->hmm.K*ctx->hmm.KS;
 			// the first call checks CM for all three (the occupancy query and the launch use the same CM)
 			if (!mb_post_sm_dispatch(mega, dump, CM, 2, dim3(), 0, ks, nullptr, &smem_static))
 				return mb_fail(ctx, MB200_EINVAL, "k_posterior_sm has no instantiation for size class %d", CM);
 			smem = (size_t) smem_static + (size_t)((tsize + 3) & ~3)*sizeof(float)
-			  + (size_t) MB_WARPS_PER_BLOCK*(mega ? 7 : 6)*CM*32*sizeof(float);
+			  + (size_t) MB_WARPS_PER_BLOCK*(mega ? MB_SM_ARRAYS_MEGA : MB_SM_ARRAYS)*CM*32*sizeof(float);
 			if (ctx->occ_cache_k != tsize*2 + (mega ? 1 : 0))
 				{
 				memset(ctx->occ_cache, 0, sizeof ctx->occ_cache);

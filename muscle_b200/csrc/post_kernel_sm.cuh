@@ -21,8 +21,9 @@
 // cache (a register-resident, fully unrolled variant stalls on instruction fetch).  Only the
 // Forward M-state is spilled (4 B/cell), in [step][c][lane] order so that both the Forward write
 // and the Backward read are full 128-byte lines.  Backward walks the same anti-diagonals in
-// reverse, fuses the Fwd (*) Bwd posterior, thresholds at log(0.01) and appends survivors to a
-// per-row candidate list; the warp then compacts the rows into MySparseMx order and runs the
+// reverse, fuses the Fwd (*) Bwd posterior score, thresholds it at log(0.01) and appends the scores of
+// survivors to a per-row candidate list; the warp then turns the scores into probabilities 32 at a time,
+// compacts the rows into MySparseMx order and runs the
 // expected-accuracy max-sum DP row by row as a warp-wide prefix-max (new[j] = max_{k<=j}
 // max(old[k], old[k-1]+P[k]) is exactly the reference's max3 recurrence because every value is an
 // exact max of the same sums).
@@ -52,10 +53,13 @@
 #pragma once
 #include "common.cuh"
 
-#define MB_SM_ARRAYS 6            // words of state per (column, lane): float4 state + {ycode, eY}  (+1 in MEGA mode: letters 4..7)
+// resident CTAs/SM the register budget is tuned for (64K registers: <= 85 per thread at 6, <= 102 at 5).
+// At 5 words per (column, lane) six CTAs of the classes up to 12 fit in an SM's shared memory; 14 and 16
+// do not, so they keep the budget of 5.
 #ifndef MB_SM_BLOCKS
-#define MB_SM_BLOCKS 5            // resident CTAs/SM the register budget is tuned for (64K registers: <= 102 per thread)
+#define MB_SM_BLOCKS 6
 #endif
+#define MB_SM_BLOCKS_WIDE 5
 #ifndef MB_SM_UNROLL
 #define MB_SM_UNROLL 1            // the rolled loop stays in the instruction cache
 #endif
@@ -86,30 +90,41 @@ __device__ __forceinline__ float mb_mega_emit(const float *T, const uint32_t (&x
 
 // CM: size class (columns per lane the shared memory is sized for; P.cmax <= CM caps C at run time)
 template <bool MEGA, int CM, bool DUMP>
-__global__ void __launch_bounds__(32*MB_WARPS_PER_BLOCK, MEGA ? 4 : MB_SM_BLOCKS)
+__global__ void __launch_bounds__(32*MB_WARPS_PER_BLOCK, MEGA ? 4 : (CM <= 12 ? MB_SM_BLOCKS : MB_SM_BLOCKS_WIDE))
 k_posterior_sm(const PostParams P)
 	{
-	constexpr int NARR = MEGA ? MB_SM_ARRAYS + 1 : MB_SM_ARRAYS;
+	constexpr int NARR = MEGA ? MB_SM_ARRAYS_MEGA : MB_SM_ARRAYS;
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	PostSmemHdr &sm = *reinterpret_cast<PostSmemHdr *>(smem_raw);
 	const MbHmm h = P.h;
 	const int lane = threadIdx.x & 31;
 	const int wib = threadIdx.x >> 5;
 	const int gwarp = blockIdx.x*MB_WARPS_PER_BLOCK + wib;
+	// plain mode: {match[x][y], ins[y]} pairs in rows of KS, so that one 64-bit load gives both emissions of
+	// a column and the per-column record holds only the class of Y; MEGA: the feature tables
 	float *matchT = reinterpret_cast<float *>(smem_raw + sizeof(PostSmemHdr));
-	const int tsize = MEGA ? (int) P.mega_tsize : h.K*h.KS;
+	float2 *meT = reinterpret_cast<float2 *>(matchT);
+	const int tsize = MEGA ? (int) P.mega_tsize : 2*h.K*h.KS;          // floats
 	float *wbase = matchT + ((tsize + 3) & ~3) + (size_t) wib*NARR*CM*32;
-	float4   *st = reinterpret_cast<float4 *>(wbase);                  // Forward {S, M, IX, JX}; Backward {M, IX, JX, -}
-	uint2    *ye = reinterpret_cast<uint2 *>(wbase + 4*CM*32);         // {class (MEGA: letters 0..3), bits of eY}
-	uint32_t *y2 = reinterpret_cast<uint32_t *>(wbase + 6*CM*32);      // MEGA only: letters 4..7
-	(void) y2;
+	float4   *st = reinterpret_cast<float4 *>(wbase);                  // Forward {S, M, IX, JX}; Backward {M, IX, JX, posterior score}
+	uint2    *ye = reinterpret_cast<uint2 *>(wbase + 4*CM*32);         // MEGA only: {letters 0..3, bits of eY}
+	uint32_t *y2 = reinterpret_cast<uint32_t *>(wbase + (MEGA ? 6 : 4)*CM*32);   // MEGA: letters 4..7; plain: class of Y
+	(void) ye;
 
 	mb_logadd_fill(sm.coef, &sm.labase);
 	if (!MEGA)
+		{
 		for (int k = threadIdx.x; k < h.K; k += blockDim.x)
 			sm.insT[k] = P.insT[k];
-	for (int k = threadIdx.x; k < tsize; k += blockDim.x)
-		matchT[k] = P.matchT[k];
+		for (int k = threadIdx.x; k < h.K*h.KS; k += blockDim.x)
+			{
+			const int b = k % h.KS;                   // columns K..KS-1 pad the row and are never read
+			meT[k] = make_float2(P.matchT[k], b < h.K ? P.insT[b] : 0.0f);
+			}
+		}
+	else
+		for (int k = threadIdx.x; k < tsize; k += blockDim.x)
+			matchT[k] = P.matchT[k];
 	const int nf = (int) P.mega_nf;
 	__syncthreads();
 
@@ -163,8 +178,6 @@ k_posterior_sm(const PostParams P)
 		const int lcl = (LY - 1 - lastj0)/C;              // lane / local column of DP column LY
 		const int clast = (LY - 1 - lastj0) - lcl*C;
 
-		for (int k = lane; k < sumLX; k += 32)
-			rowcnt[k] = 0;
 		for (int k = 0; k < nch; ++k)
 			ckept[k*32 + lane] = 0;
 
@@ -196,7 +209,7 @@ k_posterior_sm(const PostParams P)
 				else
 					{
 					const int code = jj < LY ? (int) Yc[jj] : h.pad;
-					ye[c*32 + lane] = make_uint2((uint32_t) code, __float_as_uint(sm.insT[code]));
+					y2[c*32 + lane] = (uint32_t) code;
 					}
 				st[c*32 + lane] = make_float4(Z, Z, Z, Z);
 				}
@@ -264,7 +277,7 @@ k_posterior_sm(const PostParams P)
 					dprev = Ls;
 					float lm = Lm, laiy = Laiy, lajy = Lajy, sLast = Z;
 					float ix = Z, jx = Z, iy = Z, jy = Z;
-					const float *mrow = matchT + (MEGA ? 0 : xc*h.KS);
+					const float2 *merow = meT + (MEGA ? 0 : xc*h.KS);
 					uint32_t xb[8];
 					if (MEGA)
 						{
@@ -282,9 +295,18 @@ MB_UNROLL(MB_SM_UNROLL)
 					for (int c = 0; c < cn; ++c, sp += 32, yp += 32, y2p += 32, dst += 32)
 						{
 						const float4 v = *sp;                      // {S, M, IX, JX} of row i-1
-						const uint2 y = *yp;
-						const float eyc = __uint_as_float(y.y);
-						const float em = MEGA ? mb_mega_emit(matchT, xb, y.x, *y2p, nf) : mrow[y.x];
+						float em, eyc;
+						if (MEGA)
+							{
+							const uint2 y = *yp;
+							eyc = __uint_as_float(y.y);
+							em = mb_mega_emit(matchT, xb, y.x, *y2p, nf);
+							}
+						else
+							{
+							const float2 e2 = merow[*y2p];
+							em = e2.x; eyc = e2.y;
+							}
 						const float m = ADD(diag, em);
 						ix = ADD(la(ADD(v.z, h.tII), ADD(v.y, h.tMI)), ex);
 						jx = ADD(la(ADD(v.w, h.tJJ), ADD(v.y, h.tMJ)), ex);
@@ -350,6 +372,19 @@ MB_UNROLL(MB_SM_UNROLL)
 		// The chain's pairs last to first, rows LX..1 of a pair and then a separator step; pair k starts
 		// at chain step (sum over later pairs of (LX + 1)) + nl-1-l.  ckept[k][l] counts the lane's
 		// kept entries up to the end of pair k, so that each pair's count is a difference.
+		// The column loop only tests the score: it keeps the score in the spare .w of the state record and
+		// sets bit c of a per-lane mask.  After the loop each lane appends its survivors {score, column},
+		// so the warp runs that code as often as the most survivors in one lane, not once per column in
+		// which any lane has one (under SIMT a branch costs the whole warp when one lane takes it).  The
+		// list holds scores, not probabilities: expf is a long FP64 chain, and the compaction forms p
+		// from 32 converged lanes instead.  A candidate is kept when p >= 0.01f (mysparsemx.cpp:139-141),
+		// and for every float s in [-10, 0] glibc's expf(s) >= 0.01f exactly when s >= -4.60517025f
+		// (0xc0935d8e, itself logf(0.01f); checked on all 1.09e9 of them), so the kept count is a compare
+		// of the score.  Row i's entry count travels with the wavefront like the state: lane l+1 finished
+		// its columns of row i, which lie to the right, one step before lane l, so the list stays in
+		// descending column order; across strips the count rides in the spare .w of the edge record, and
+		// lane 0 of strip 0, the last to touch the row, stores it in rowcnt.
+		const float keepScore = fmaxf(h.minScore, __uint_as_float(0xc0935d8eu));
 		uint32_t kept = 0;
 		bool overflow = false;
 		for (int strip = nstrips - 1; strip >= 0; --strip)
@@ -375,11 +410,12 @@ MB_UNROLL(MB_SM_UNROLL)
 				else
 					{
 					const int code = jj < LY ? (int) Yc[jj] : h.pad;
-					ye[c*32 + lane] = make_uint2((uint32_t) code, __float_as_uint(sm.insT[code]));
+					y2[c*32 + lane] = (uint32_t) code;
 					}
 				st[c*32 + lane] = make_float4(Z, Z, Z, Z);
 				}
 			float outM = Z, outIY = Z, outJY = Z;
+			uint32_t outCnt = 0;
 			float dprev = Z;
 			const int nsteps = sumLX + nch - 2 + nl;
 			int xcPref = h.pad;
@@ -408,22 +444,23 @@ MB_UNROLL(MB_SM_UNROLL)
 				float Rm = __shfl_down_sync(MB_FULL, outM, 1);
 				float Riy = __shfl_down_sync(MB_FULL, outIY, 1);
 				float Rjy = __shfl_down_sync(MB_FULL, outJY, 1);
+				uint32_t cnt = __shfl_down_sync(MB_FULL, outCnt, 1);    // entries already in the row
 				if (i >= 1 && i <= LX && lane < nl)
 					{
 					if (lane == nl - 1)
 						{
 						if (last)
 							{
-							Rm = Z; Riy = Z; Rjy = Z;
+							Rm = Z; Riy = Z; Rjy = Z; cnt = 0;
 							}
 						else
 							{
 							const float4 e = edgeIn[i];
-							Rm = e.x; Riy = e.y; Rjy = e.z;
+							Rm = e.x; Riy = e.y; Rjy = e.z; cnt = __float_as_uint(e.w);
 							}
 						}
 					const float ex = MEGA ? exm : sm.insT[xc];
-					const float *mrow = matchT + (MEGA ? 0 : xc*h.KS);
+					const float2 *merow = meT + (MEGA ? 0 : xc*h.KS);
 					uint32_t xb[8];
 					if (MEGA)
 						{
@@ -431,37 +468,25 @@ MB_UNROLL(MB_SM_UNROLL)
 						for (int f = 0; f < 8; ++f)
 							xb[f] = P.mega_base[f] + ((f < 4 ? (xl.x >> (8*f)) : (xl.y >> (8*(f - 4)))) & 255u)*P.mega_alpha[f];
 						}
-					uint32_t cnt = rowcnt[rk + i - 1];
-					const uint32_t cnt0 = cnt;
-					mb200_entry *row = rows + (size_t)(rk + i - 1)*MB_CAP;
 					const int t = fk + i + lane;
 					const int col0 = j0 + lane*C;
 					float mdiag = dprev;
 					dprev = Rm;
 					float riy = Riy, rjy = Rjy, mFirst = Z;
-					// posterior (calcposteriorflat.cpp:14-22); candidates arrive with descending column
+					// posterior score (calcposteriorflat.cpp:14-22) and its threshold; columns arrive descending,
+					// so bit c of hits ends up on column c
+					uint32_t hits = 0;
 					auto post = [&](int c, float fmv, float m)
 						{
 						const float score = __fsub_rn(ADD(fmv, m), total);
-						if (score >= h.minScore)
-							{
-							const float p = score >= 0.0f ? 1.0f : mb_expf_glibc(score);
-							if (cnt < MB_CAP)
-								{
-								row[cnt].p = p;
-								row[cnt].col = (uint32_t)(col0 + c);
-								}
-							else
-								overflow = true;
-							++cnt;
-							kept += (p >= 0.01f) ? 1u : 0u;
-							}
+						hits = 2u*hits + (score >= h.minScore ? 1u : 0u);
 						if (DUMP && cpairs[kp] == P.dbg_pair)
 							{
 							P.dbg_bwd[(size_t)(i - 1)*LY + col0 + c] = m;
 							P.dbg_post[(size_t)(i - 1)*LY + col0 + c] =
 							  score < h.minScore ? 0.0f : (score >= 0.0f ? 1.0f : mb_expf_glibc(score));
 							}
+						return score;
 						};
 					float4 *sp = st + lane;
 					const uint2 *yp = ye + lane;
@@ -474,25 +499,38 @@ MB_UNROLL(MB_SM_UNROLL)
 						{
 						// cell (LX,LY), the lane's first: the end scores (bwdflat3.cpp:53-61)
 						mdiag = sp->x;
-						*sp = make_float4(h.tSM, h.tSI, h.tSJ, Z);
+						*sp = make_float4(h.tSM, h.tSI, h.tSJ, post(c, *src, h.tSM));
 						riy = h.tSI; rjy = h.tSJ; mFirst = h.tSM;
-						post(c, *src, h.tSM);
 						--c; sp -= 32; yp -= 32; y2p -= 32; src -= 32;
 						}
-					// the prefetch reads src[-32] when c reaches 0, unguarded: it is inside this warp's spill (t >= 1),
-					// and since t is the same in every lane it is step t-1's column C-1, the line this warp loads
-					// first in its next step, so it adds no line of traffic
-					float fmNext = *src;
+					// Forward M is loaded two columns ahead.  ptxas places the load where register pressure lets
+					// it, mid-loop here; one column ahead that left less than an iteration to cover an HBM miss and
+					// cost C4 6 % (the CM = 16 class runs 4 warps per scheduler).  The loads stay within this step's
+					// columns, except *src when the cell (LX,LY) was the lane's only column (c = -1): that is
+					// step t-1's column C-1 (t is the same in every lane), inside this warp's spill since t >= 1
+					float fmNext = *src;                       // column c
+					float fmNext2 = c >= 1 ? src[-32] : 0.0f;  // column c-1
 MB_UNROLL(MB_SM_UNROLL)
 					for (; c >= 0; --c, sp -= 32, yp -= 32, y2p -= 32)
 						{
 						const float fmv = fmNext;
+						fmNext = fmNext2;
 						src -= 32;
-						fmNext = *src;
-						const float4 v = *sp;                      // {M, IX, JX, -} of row i+1
-						const uint2 y = *yp;
-						const float eyc = __uint_as_float(y.y);
-						const float em = MEGA ? mb_mega_emit(matchT, xb, y.x, *y2p, nf) : mrow[y.x];
+						if (c >= 2)
+							fmNext2 = src[-32];                // column c-2
+						const float4 v = *sp;                      // {M, IX, JX, score} of row i+1
+						float em, eyc;
+						if (MEGA)
+							{
+							const uint2 y = *yp;
+							eyc = __uint_as_float(y.y);
+							em = mb_mega_emit(matchT, xb, y.x, *y2p, nf);
+							}
+						else
+							{
+							const float2 e2 = merow[*y2p];
+							em = e2.x; eyc = e2.y;
+							}
 						const float nM = ADD(mdiag, em);
 						const float nIX = ADD(v.y, ex);
 						const float nJX = ADD(v.z, ex);
@@ -505,16 +543,34 @@ MB_UNROLL(MB_SM_UNROLL)
 						const float iy = la(ADD(h.tII, nIY), ADD(h.tIM, nM));
 						const float jy = la(ADD(h.tJJ, nJY), ADD(h.tJM, nM));
 						mdiag = v.x;
-						*sp = make_float4(m, ix, jx, Z);
+						*sp = make_float4(m, ix, jx, post(c, fmv, m));
 						riy = iy; rjy = jy;
 						mFirst = m;
-						post(c, fmv, m);
+						}
+					// the survivors, highest column first (the row's order): the warp runs this loop as often as
+					// the most survivors in one lane, not once per column in which any lane has one
+					mb200_entry *row = rows + (size_t)(rk + i - 1)*MB_CAP;
+					while (hits)
+						{
+						const int hc = 31 - __clz(hits);
+						hits ^= 1u << hc;
+						const float score = st[hc*32 + lane].w;
+						if (cnt < MB_CAP)
+							*reinterpret_cast<uint2 *>(row + cnt) = make_uint2(__float_as_uint(score), (uint32_t)(col0 + hc));
+						else
+							overflow = true;
+						++cnt;
+						kept += score >= keepScore ? 1u : 0u;
 						}
 					outM = mFirst; outIY = riy; outJY = rjy;
-					if (lane == 0 && strip > 0)
-						edgeOut[i] = make_float4(outM, outIY, outJY, 0.0f);
-					if (cnt != cnt0)
-						rowcnt[rk + i - 1] = (uint8_t) min(cnt, (uint32_t) MB_CAP);
+					outCnt = cnt;
+					if (lane == 0)
+						{
+						if (strip > 0)
+							edgeOut[i] = make_float4(outM, outIY, outJY, __uint_as_float(cnt));
+						else
+							rowcnt[rk + i - 1] = (uint8_t) min(cnt, (uint32_t) MB_CAP);
+						}
 					}
 				else if (i == 0 && lane < nl)         // separator, then the previous pair of the chain
 					{
@@ -522,6 +578,7 @@ MB_UNROLL(MB_SM_UNROLL)
 					for (int c = 0; c < C; ++c)
 						st[c*32 + lane] = make_float4(Z, Z, Z, Z);
 					outM = Z; outIY = Z; outJY = Z;
+					outCnt = 0;
 					dprev = Z;
 					ckept[kp*32 + lane] = kept;
 					if (kp > 0)
@@ -599,7 +656,10 @@ MB_UNROLL(MB_SM_UNROLL)
 						const int idx = (int) cnt - 1 - (int)(e0 + lane);
 						mb200_entry ent; ent.p = 0.0f; ent.col = 0;
 						if (idx >= 0)
-							ent = row[idx];
+							{
+							ent = row[idx];             // {score, column}: the probability (calcposteriorflat.cpp:20)
+							ent.p = ent.p >= 0.0f ? 1.0f : mb_expf_glibc(ent.p);
+							}
 						const int lc = (int) ent.col - j0;
 						if (idx >= 0 && lc >= 0 && lc < W)
 							rowbuf[lc] = ent.p;
