@@ -184,6 +184,23 @@ class Oracle:
 		self.lib.mo_conspair(n, _p(lens, u32p), x, y, rop, enp, C.c_void_p(out.ctypes.data))
 		return out
 
+	def conspair_many(self, lens, pairs, row_off, entries):
+		"""conspair of every (x, y) in pairs, with the per-pair pointer arrays built once -> list of entries"""
+		n = len(lens)
+		npairs = n*(n - 1)//2
+		lens = np.ascontiguousarray(lens, np.uint32)
+		ro = [np.ascontiguousarray(a, np.uint32) for a in row_off]
+		en = [np.ascontiguousarray(a, ENTRY) for a in entries]
+		rop = (u32p*npairs)(*[_p(a, u32p) for a in ro])
+		enp = (C.c_void_p*npairs)(*[a.ctypes.data for a in en])
+		outs = []
+		for x, y in pairs:
+			p = x*n - x*(x + 1)//2 + (y - x - 1)
+			out = np.empty(len(en[p]), ENTRY)
+			self.lib.mo_conspair(n, _p(lens, u32p), x, y, rop, enp, C.c_void_p(out.ctypes.data))
+			outs.append(out)
+		return outs
+
 	def buildpost(self, lens, ids_a, p2c_a, cols_a, ids_b, p2c_b, cols_b, row_off, entries):
 		n = len(lens)
 		npairs = n*(n - 1)//2

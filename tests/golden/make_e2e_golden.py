@@ -73,7 +73,29 @@ def profalign():
 	  "-output", os.path.join(OUT, "profalign.ref.afa"), "-quiet"], check=True)
 
 
+def repeats():
+	"""rep16: 16 proteins of one family, each with a tandem-repeat region (QQQP, PPG or SG, 20-86 residues,
+	3 % substitutions) in its middle, whose posterior rows hold up to 42 entries >= 0.01"""
+	sys.path.insert(0, os.path.join(ROOT, "tests"))
+	import numpy as np
+	import repeat_util as ru
+	seqs = synth.make_family(16, 150, 20, seed=105)
+	rng = np.random.default_rng(105)
+	for k, s in enumerate(seqs):
+		rep = ru.mutate(rng, ru.tandem(ru.MOTIFS[k % 3], 20 + (11*k) % 67, k % 4), 0.03)
+		seqs[k] = s[:len(s)//2] + rep + s[len(s)//2:]
+	fa = os.path.join(OUT, "rep16.fa")
+	with open(fa, "w") as f:
+		for i, s in enumerate(seqs):
+			f.write(">s%d\n%s\n" % (i, s))
+	subprocess.run([CLI, "-align", fa, "-output", os.path.join(OUT, "rep16.ref.afa"), "-quiet"], check=True)
+
+
 if __name__ == "__main__":
+	if sys.argv[1:] == ["repeats"]:
+		repeats()
+		sys.exit()
 	super5()
 	main()
 	profalign()
+	repeats()

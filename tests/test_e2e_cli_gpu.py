@@ -45,7 +45,7 @@ def pair_set(rows):
 	return out
 
 
-@pytest.mark.parametrize("name", ["fam12", "fam30", "fam6_long"])
+@pytest.mark.parametrize("name", ["fam12", "fam30", "fam6_long", "rep16"])
 def test_align_cli_matches_reference_msa(name, tmp_path):
 	if not os.path.exists(CLI):
 		pytest.skip("integration/_build/muscle_b200 not built (needs oracle/_ref built from the reference sources)")
