@@ -145,6 +145,14 @@ __device__ __forceinline__ float mb_expf_glibc(float x)
 	return __double2float_rn(y);
 	}
 
+// head of k_posterior_sm's dynamic shared memory; the emission tables and the warps' state follow it
+struct PostSmemHdr
+	{
+	float4   coef[17];    // LOGEXP1 pieces indexed by ceil(2*gap), see LogAdd
+	float    insT[MB_MAX_K];
+	uint32_t labase;      // biased shared address of coef (mb_logadd_make)
+	};
+
 struct PostParams
 	{
 	MbHmm h;

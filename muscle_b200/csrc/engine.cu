@@ -62,11 +62,8 @@ void DevBuf::release()
 // both stages of a 1000-protein problem fit one 80 GB device.  The next posterior call reallocates it.
 void mb_release_post_scratch(mb200_ctx *ctx)
 	{
-	for (int c = 0; c <= MB_MAX_C; ++c)
-		{
-		ctx->d_fm[c].release(); ctx->d_edge[c].release(); ctx->d_rows[c].release(); ctx->d_rowcnt[c].release();
-		ctx->d_chainbuf[c].release();
-		}
+	for (DevBuf &b : ctx->d_post_scratch)
+		b.release();
 	}
 
 #define ENSURE(buf, bytes) do { if ((buf).ensure(bytes) != 0) \
@@ -559,30 +556,30 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 			const uint32_t lxmax = ctx->plan_lxmax[C], lymax = ctx->plan_lymax[C];
 			const uint32_t W = 32u*C;
 			const uint32_t nstrips = (lymax + W - 1)/W;
-			int smem_static = 0, occ = 0;
-			size_t smem;
+			int occ = 0;
 			const bool mega = ctx->mega;
 			const bool dump = dbg != nullptr;
 			const int CM = mb_post_sm_class(C);      // == C unless the width is forced
+			const void *kern = mb_post_sm_kernel(mega, dump, CM);
+			if (!kern)
+				return mb_fail(ctx, MB200_EINVAL, "k_posterior_sm has no instantiation for size class %d", CM);
 			// floats of the emission table in shared memory (plain mode: {match, ins} pairs, see k_posterior_sm)
 			const int tsize = mega ? (int) ctx->mega_tsize : 2*ctx->hmm.K*ctx->hmm.KS;
-			// the first call checks CM for all three (the occupancy query and the launch use the same CM)
-			if (!mb_post_sm_dispatch(mega, dump, CM, 2, dim3(), 0, ks, nullptr, &smem_static))
-				return mb_fail(ctx, MB200_EINVAL, "k_posterior_sm has no instantiation for size class %d", CM);
-			smem = (size_t) smem_static + (size_t)((tsize + 3) & ~3)*sizeof(float)
+			const size_t smem = sizeof(PostSmemHdr) + (size_t)((tsize + 3) & ~3)*sizeof(float)
 			  + (size_t) MB_WARPS_PER_BLOCK*(mega ? MB_SM_ARRAYS_MEGA : MB_SM_ARRAYS)*CM*32*sizeof(float);
+			CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
 			if (ctx->occ_cache_k != tsize*2 + (mega ? 1 : 0))
 				{
 				memset(ctx->occ_cache, 0, sizeof ctx->occ_cache);
 				ctx->occ_cache_k = tsize*2 + (mega ? 1 : 0);
 				}
 			if (dump)          // another instantiation: not cached
-				mb_post_sm_dispatch(mega, dump, CM, 1, dim3(), smem, ks, nullptr, &occ);
+				CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 32*MB_WARPS_PER_BLOCK, smem));
 			else
 				{
 				if (ctx->occ_cache[C] == 0)
 					{
-					mb_post_sm_dispatch(mega, dump, CM, 1, dim3(), smem, ks, nullptr, &occ);
+					CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 32*MB_WARPS_PER_BLOCK, smem));
 					ctx->occ_cache[C] = occ;
 					}
 				occ = ctx->occ_cache[C];
@@ -605,23 +602,26 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 			P.edge_stride = 2*((size_t) lxmax + 2);
 			P.rows_stride = (size_t) ctx->plan_rmax[C]*MB_CAP;
 			P.rowcnt_stride = ((size_t) ctx->plan_rmax[C] + 31)/16*16;
-			size_t per_warp = P.fm_stride*4 + P.edge_stride*16 + P.rows_stride*8 + P.rowcnt_stride + MB_CHAIN_BUF*4;
+			// bytes per warp of the arrays fm, edge, rows, rowcnt and chainbuf
+			const size_t bytes[5] = { P.fm_stride*4, P.edge_stride*16, P.rows_stride*8, P.rowcnt_stride,
+			  (size_t) MB_CHAIN_BUF*4 };
+			const size_t per_warp = bytes[0] + bytes[1] + bytes[2] + bytes[3] + bytes[4];
 			if (free_b == 0)
 				cudaMemGetInfo(&free_b, &total_b);
-			const size_t held = ctx->d_fm[C].cap + ctx->d_edge[C].cap + ctx->d_rows[C].cap + ctx->d_rowcnt[C].cap
-			  + ctx->d_chainbuf[C].cap;
+			DevBuf &scratch = ctx->d_post_scratch[C];
+			const size_t held = scratch.cap;
 			const size_t have = free_b + held;
 			size_t use_warps = nwarps;
 			if (per_warp*use_warps > have*8/10)
 				use_warps = std::max<size_t>(MB_WARPS_PER_BLOCK, (have*8/10/per_warp)/MB_WARPS_PER_BLOCK*MB_WARPS_PER_BLOCK);
 			nblocks = (uint32_t)(use_warps/MB_WARPS_PER_BLOCK);
-			ENSURE(ctx->d_fm[C], P.fm_stride*4*use_warps);
-			ENSURE(ctx->d_edge[C], P.edge_stride*16*use_warps);
-			ENSURE(ctx->d_rows[C], P.rows_stride*8*use_warps);
-			ENSURE(ctx->d_rowcnt[C], P.rowcnt_stride*use_warps);
-			ENSURE(ctx->d_chainbuf[C], (size_t) MB_CHAIN_BUF*4*use_warps);
-			if (ctx->d_fm[C].cap + ctx->d_edge[C].cap + ctx->d_rows[C].cap + ctx->d_rowcnt[C].cap + ctx->d_chainbuf[C].cap != held)
-				free_b = 0;                        // something was (re)allocated: ask again for the next size class
+			// one buffer holds the five arrays of all warps, each starting on a 256-byte boundary
+			size_t off[6] = {};
+			for (int a = 0; a < 5; ++a)
+				off[a + 1] = off[a] + (bytes[a]*use_warps + 255)/256*256;
+			ENSURE(scratch, off[5]);
+			if (scratch.cap != held)
+				free_b = 0;                        // it was (re)allocated: ask again for the next size class
 			P.h = ctx->hmm;
 			P.matchT = (const float *)(mega ? ctx->d_megaT.p : ctx->d_matchT.p);
 			P.insT = (const float *)(mega ? ctx->d_insP.p : ctx->d_insT.p);
@@ -637,11 +637,11 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 			P.chain = (const uint32_t *) ctx->d_chain.p + bin_start[C];
 			P.nwork = nchains;
 			P.counter = (uint32_t *)((char *) ctx->d_cursor.p + 16) + C;
-			P.fm = (float *) ctx->d_fm[C].p;
-			P.edge = (float4 *) ctx->d_edge[C].p;
-			P.rows = (mb200_entry *) ctx->d_rows[C].p;
-			P.rowcnt = (uint8_t *) ctx->d_rowcnt[C].p;
-			P.chainbuf = (uint32_t *) ctx->d_chainbuf[C].p;
+			P.fm = (float *)((char *) scratch.p + off[0]);
+			P.edge = (float4 *)((char *) scratch.p + off[1]);
+			P.rows = (mb200_entry *)((char *) scratch.p + off[2]);
+			P.rowcnt = (uint8_t *)((char *) scratch.p + off[3]);
+			P.chainbuf = (uint32_t *)((char *) scratch.p + off[4]);
 			P.rowoff = (uint32_t *) ctx->d_rowoff.p;
 			P.rowbase = (const uint64_t *) ctx->d_rowbase.p;
 			P.entries = (mb200_entry *) ctx->d_entries.p;
@@ -657,8 +657,8 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 				P.dbg_pair = dbg->pair;
 				}
 			P.cmax = (uint32_t) C;
-			mb_post_sm_dispatch(mega, dump, CM, 0, dim3(nblocks), smem, ks, &P, nullptr);
-			CU(cudaGetLastError());
+			void *args[] = { &P };
+			CU(cudaLaunchKernel(kern, dim3(nblocks), dim3(32*MB_WARPS_PER_BLOCK), args, smem, ks));
 			ctx->stats.kernel_launches++;
 			}
 		for (int k = 0; k < mb200_ctx::kStreams; ++k)
@@ -706,11 +706,9 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 	return MB200_OK;
 	}
 
-int mb200_posteriors(mb200_ctx *ctx, uint32_t npairs, const uint32_t *pair_x, const uint32_t *pair_y,
-  uint32_t flags, float *ea_out)
+// a pair list given by the caller: the store no longer holds it, and the plan is rebuilt for it
+static void install_pairs(mb200_ctx *ctx, uint32_t npairs, const uint32_t *pair_x, const uint32_t *pair_y)
 	{
-	if (!ctx || npairs == 0 || !pair_x || !pair_y)
-		return mb_fail(ctx, MB200_EINVAL, "mb200_posteriors: bad argument");
 	ctx->h_px.assign(pair_x, pair_x + npairs);
 	ctx->h_py.assign(pair_y, pair_y + npairs);
 	ctx->store_allpairs = false;
@@ -718,6 +716,14 @@ int mb200_posteriors(mb200_ctx *ctx, uint32_t npairs, const uint32_t *pair_x, co
 	ctx->store_valid = false;
 	ctx->plan_valid = false;
 	ctx->plan_is_allpairs = false;
+	}
+
+int mb200_posteriors(mb200_ctx *ctx, uint32_t npairs, const uint32_t *pair_x, const uint32_t *pair_y,
+  uint32_t flags, float *ea_out)
+	{
+	if (!ctx || npairs == 0 || !pair_x || !pair_y)
+		return mb_fail(ctx, MB200_EINVAL, "mb200_posteriors: bad argument");
+	install_pairs(ctx, npairs, pair_x, pair_y);
 	const int force_c = (int)((flags >> 8) & 0xff);
 	if (force_c > MB_MAX_C)
 		return mb_fail(ctx, MB200_EINVAL, "forced C %d > %d", force_c, MB_MAX_C);
@@ -777,8 +783,6 @@ int mb200_posteriors_allpairs(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi, floa
 		{
 		ctx->store_allpairs = (p_lo == 0 && p_hi == npairs);
 		ctx->ea_allpairs = ctx->store_allpairs;
-		ctx->store_p_lo = p_lo;
-		ctx->store_p_hi = p_hi;
 		}
 	return rc;
 	}
@@ -794,13 +798,7 @@ int mb200_calc_post_dense_pair(mb200_ctx *ctx, uint32_t npairs, const uint32_t *
 	ENSURE(ctx->d_dbg, (3*n + 4)*sizeof(float));
 	float *base = (float *) ctx->d_dbg.p;
 	PostDebug dbg = { base, base + n, base + 2*n, base + 3*n, which };
-	ctx->h_px.assign(pair_x, pair_x + npairs);
-	ctx->h_py.assign(pair_y, pair_y + npairs);
-	ctx->store_allpairs = false;
-	ctx->ea_allpairs = false;
-	ctx->store_valid = false;
-	ctx->plan_valid = false;
-	ctx->plan_is_allpairs = false;
+	install_pairs(ctx, npairs, pair_x, pair_y);
 	const int rc = run_posteriors(ctx, nullptr, &dbg, ctx->debug_force_c);
 	if (rc != MB200_OK)
 		return rc;

@@ -86,9 +86,8 @@ struct mb200_ctx
 	std::vector<uint32_t> plan_bin_start, plan_lxmax, plan_lymax;  // bin_start: first chain of each size class
 	std::vector<uint64_t> plan_fmax, plan_rmax;                    // largest chain: Forward rows (sum of LX+2), rows (sum of LX)
 
-	// per-warp scratch of the posterior kernel
-	DevBuf d_fm[MB_MAX_C + 1], d_edge[MB_MAX_C + 1], d_rows[MB_MAX_C + 1], d_rowcnt[MB_MAX_C + 1];   // per bin
-	DevBuf d_chainbuf[MB_MAX_C + 1];
+	// per-warp scratch of the posterior kernel, one buffer per bin (PostParams fm, edge, rows, rowcnt, chainbuf)
+	DevBuf d_post_scratch[MB_MAX_C + 1];
 	static constexpr int kStreams = 4;          // column-width bins run concurrently to overlap their tails
 	cudaStream_t aux[kStreams] = {};
 	cudaEvent_t aux_done[kStreams] = {};

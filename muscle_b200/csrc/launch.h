@@ -10,8 +10,7 @@ static inline int mb_post_sm_class(int C)
 	{
 	return C <= 12 ? (C + 3)/4*4 : (C <= 14 ? 14 : 16);
 	}
-// op 0: launch, 1: occupancy (blocks/SM) -> *out, 2: static smem struct bytes -> *out.
-// dump: the instantiation that writes the dense debug arrays of PostParams (mb200_calc_post_dense).
-// Returns false if cm is not a size class.
-bool mb_post_sm_dispatch(bool mega, bool dump, int cm, int op, dim3 grid, size_t smem, cudaStream_t st,
-  const PostParams *P, int *out);
+// The k_posterior_sm instantiation for size class cm, launched with one PostParams argument; nullptr if
+// cm is not a size class.  dump: the instantiation that writes the dense debug arrays of PostParams
+// (mb200_calc_post_dense).
+const void *mb_post_sm_kernel(bool mega, bool dump, int cm);

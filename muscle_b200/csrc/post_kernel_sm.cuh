@@ -56,22 +56,8 @@
 // resident CTAs/SM the register budget is tuned for (64K registers: <= 85 per thread at 6, <= 102 at 5).
 // At 5 words per (column, lane) six CTAs of the classes up to 12 fit in an SM's shared memory; 14 and 16
 // do not, so they keep the budget of 5.
-#ifndef MB_SM_BLOCKS
 #define MB_SM_BLOCKS 6
-#endif
 #define MB_SM_BLOCKS_WIDE 5
-#ifndef MB_SM_UNROLL
-#define MB_SM_UNROLL 1            // the rolled loop stays in the instruction cache
-#endif
-#define MB_PRAGMA(x) _Pragma(#x)
-#define MB_UNROLL(n) MB_PRAGMA(unroll n)
-
-struct PostSmemHdr
-	{
-	float4   coef[17];    // LOGEXP1 pieces indexed by ceil(2*gap), see LogAdd
-	float    insT[MB_MAX_K];
-	uint32_t labase;      // biased shared address of coef (mb_logadd_make)
-	};
 
 // sum over features of the pre-multiplied pair tables, in feature order starting from 0
 // (mega.cpp:350-357); xb[f] = offset of row a_f of feature f's table, y0/y1 = packed letters of the column
@@ -86,6 +72,282 @@ __device__ __forceinline__ float mb_mega_emit(const float *T, const uint32_t (&x
 	if (nf > 6) e = ADD(e, T[xb[6] + ((y1 >> 16) & 255u)]);
 	if (nf > 7) e = ADD(e, T[xb[7] + (y1 >> 24)]);
 	return e;
+	}
+
+
+// a sequence as the kernel reads it: residue classes (plain), or 8 letter bytes and the insert emission
+// of every position (MEGA)
+struct MbSeq
+	{
+	int len;
+	const uint8_t *code;
+	const uint2 *letters;
+	const float *ins;
+	};
+
+__device__ __forceinline__ MbSeq mb_seq(const PostParams &P, uint32_t s)
+	{
+	const uint64_t o = P.seqoff[s];
+	return { (int) P.seqlen[s], P.codes + o, reinterpret_cast<const uint2 *>(P.codes) + o, P.insT + o };
+	}
+
+// position i of X as a row of the DP needs it (class, or letters and insert emission); the padding when
+// !in.  Loaded one step ahead of its use.
+struct MbXRow { int code; uint2 letters; float ins; };
+
+template <bool MEGA>
+__device__ __forceinline__ MbXRow mb_x_row(const MbSeq &X, bool in, int i, int pad)
+	{
+	MbXRow r = { pad, make_uint2(0u, 0u), 0.0f };
+	if (MEGA)
+		{
+		r.letters = in ? X.letters[i] : make_uint2(0u, 0u);
+		r.ins = in ? X.ins[i] : 0.0f;
+		}
+	else
+		r.code = in ? (int) X.code[i] : pad;
+	return r;
+	}
+
+// X's side of the emissions of a row: its insert emission, and its {match, insert} table row merow
+// (plain) or xb of mb_mega_emit for its letters (MEGA)
+struct MbXEmit { float ins; const float2 *merow; uint32_t xb[8]; };
+
+template <bool MEGA>
+__device__ __forceinline__ MbXEmit mb_x_emit(const PostParams &P, const float *insT, const float2 *meT, int KS,
+  const MbXRow &x)
+	{
+	MbXEmit e;
+	e.ins = MEGA ? x.ins : insT[x.code];
+	e.merow = meT + (MEGA ? 0 : x.code*KS);
+	if (MEGA)
+		{
+#pragma unroll
+		for (int f = 0; f < 8; ++f)
+			e.xb[f] = P.mega_base[f]
+			  + ((f < 4 ? (x.letters.x >> (8*f)) : (x.letters.y >> (8*(f - 4)))) & 255u)*P.mega_alpha[f];
+		}
+	return e;
+	}
+
+// {match emission, insert emission of Y} of a column whose staged Y data is at yp / y2p, in a row with
+// X's side xe
+template <bool MEGA>
+__device__ __forceinline__ float2 mb_col_emit(const float *matchT, const MbXEmit &xe, int nf, const uint2 *yp,
+  const uint32_t *y2p)
+	{
+	if (MEGA)
+		{
+		const uint2 y = *yp;
+		return make_float2(mb_mega_emit(matchT, xe.xb, y.x, *y2p, nf), __uint_as_float(y.y));
+		}
+	return xe.merow[*y2p];
+	}
+
+// one strip of a chain: j0, the position in Y of its first column; nl, the lanes that hold columns of it;
+// cn, the lane's columns up to LY
+struct MbStrip { int j0, nl, cn; bool last; };
+
+// a chain's Y cut into n strips of W = 32*C columns, lane l holding local columns l*C .. l*C+C-1 of each;
+// DP column LY is local column clast of lane lcl in the last strip
+struct MbStrips
+	{
+	int C, W, n, lcl, clast;
+	__device__ __forceinline__ MbStrip at(int s, int lane) const
+		{
+		const bool last = s == n - 1;
+		return { s*W, last ? lcl + 1 : 32, (last && lane == lcl) ? clast + 1 : C, last };
+		}
+	};
+
+__device__ __forceinline__ MbStrips mb_strips(int LY, int C)
+	{
+	const int W = 32*C, n = (LY + W - 1)/W;
+	const int q = LY - 1 - (n - 1)*W;
+	return { C, W, n, q/C, q - q/C*C };
+	}
+
+// strip s's edge buffers: strips alternate between the two halves
+struct MbEdges { const float4 *in; float4 *out; };
+
+__device__ __forceinline__ MbEdges mb_strip_edges(float4 *edge0, float4 *edge1, int s)
+	{
+	return { (s & 1) ? edge0 : edge1, (s & 1) ? edge1 : edge0 };
+	}
+
+// the lane's C state records to LOG_ZERO: the border a pair starts from
+__device__ __forceinline__ void mb_clear_state(float4 *st, int C, int lane)
+	{
+#pragma unroll 1
+	for (int c = 0; c < C; ++c)
+		st[c*32 + lane] = make_float4(MB_LOG_ZERO, MB_LOG_ZERO, MB_LOG_ZERO, MB_LOG_ZERO);
+	}
+
+// stages Y for the lane's C columns of a strip, from position j of Y on (Backward reads the emissions of
+// the column to its right, so it passes j one higher), and clears their state records.  Positions past
+// LY get the padding class (plain) or zero letters and emission (MEGA).
+template <bool MEGA>
+__device__ __forceinline__ void mb_stage_y(const MbSeq &Y, int j, int C, int lane, int pad, float4 *st, uint2 *ye,
+  uint32_t *y2)
+	{
+	for (int c = 0; c < C; ++c, ++j)
+		{
+		const bool in = j < Y.len;
+		if (MEGA)
+			{
+			const uint2 yl = in ? Y.letters[j] : make_uint2(0u, 0u);
+			ye[c*32 + lane] = make_uint2(yl.x, __float_as_uint(in ? Y.ins[j] : 0.0f));
+			y2[c*32 + lane] = yl.y;
+			}
+		else
+			y2[c*32 + lane] = in ? (uint32_t) Y.code[j] : (uint32_t) pad;
+		}
+	mb_clear_state(st, C, lane);
+	}
+
+// Compaction and expected accuracy of one pair of a chain, once Backward has left its candidate rows (scores,
+// columns descending) at prow / pcnt: the warp turns the scores into probabilities 32 at a time, writes the
+// entries >= 0.01 in MySparseMx order with their row offsets, and runs the expected-accuracy max-sum DP
+// row by row as a warp-wide prefix-max (new[j] = max_{k<=j} max(old[k], old[k-1]+P[k])), strip by strip
+// through the edge buffers eIn / eOut.  kept: the lane's kept candidates of the pair.
+template <bool MEGA, int CM>
+__device__ void mb_compact_ea(const PostParams &P, uint32_t pair, int LX, int LY, uint32_t kept,
+  const mb200_entry *prow, const uint8_t *pcnt, const MbStrips &g, float *wbase, float *eIn, float *eOut)
+	{
+	const int lane = threadIdx.x & 31;
+	const int C = g.C, W = g.W;
+	for (int o = 16; o > 0; o >>= 1)
+		kept += __shfl_xor_sync(MB_FULL, kept, o);
+	unsigned long long base = 0;
+	if (lane == 0)
+		base = atomicAdd(P.ent_cursor, (unsigned long long) kept);
+	base = __shfl_sync(MB_FULL, base, 0);
+	const bool fits = (base + kept <= P.ent_cap);
+	if (lane == 0)
+		{
+		if (!fits)
+			atomicCAS(P.err, 0, MB200_ENOMEM);
+		P.entbase[pair] = base;
+		P.nnz[pair] = kept;
+		}
+	uint32_t *rowoff = P.rowoff + P.rowbase[pair];
+	mb200_entry *out = P.entries + base;
+
+	float eaScore = 0.0f;
+	// the warp's state area, reused as three plain float arrays of CM*32
+	float *old = wbase;                 // [c][lane]
+	float *rowbuf = wbase + CM*32;      // column-linear: [lane*C + c]
+	float *pre = wbase + 2*CM*32;       // [c][lane]
+	uint32_t written = 0;
+	for (int strip = 0; strip < g.n; ++strip)
+		{
+		const auto [j0, nl, cn, last] = g.at(strip, lane);
+		for (int c = 0; c < C; ++c)
+			{
+			old[c*32 + lane] = 0.0f;
+			rowbuf[c*32 + lane] = 0.0f;
+			}
+		__syncwarp();
+		for (int i = 1; i <= LX; ++i)
+			{
+			const uint32_t cnt = pcnt[i - 1];
+			const mb200_entry *row = prow + (size_t)(i - 1)*MB_CAP;
+			if (strip == 0 && lane == 0)
+				rowoff[i - 1] = written;
+			for (uint32_t e0 = 0; e0 < cnt; e0 += 32)
+				{
+				const int idx = (int) cnt - 1 - (int)(e0 + lane);
+				mb200_entry ent; ent.p = 0.0f; ent.col = 0;
+				if (idx >= 0)
+					{
+					ent = row[idx];             // {score, column}: the probability (calcposteriorflat.cpp:20)
+					ent.p = ent.p >= 0.0f ? 1.0f : mb_expf_glibc(ent.p);
+					}
+				const int lc = (int) ent.col - j0;
+				if (idx >= 0 && lc >= 0 && lc < W)
+					rowbuf[lc] = ent.p;
+				if (strip == 0)
+					{
+					const bool keep = idx >= 0 && ent.p >= 0.01f;          // mysparsemx.cpp:139-141
+					const uint32_t b = __ballot_sync(MB_FULL, keep);
+					if (keep && fits)
+						out[written + __popc(b & ((1u << lane) - 1u))] = ent;
+					written += __popc(b);
+					}
+				}
+			__syncwarp();
+			// calcalnscoreflat.cpp:13-29 as a prefix-max over the row
+			float leftOld = 0.0f, incoming = 0.0f;
+			if (lane == 0)
+				{
+				leftOld = strip == 0 ? 0.0f : eIn[i - 1];
+				incoming = strip == 0 ? 0.0f : eIn[i];
+				}
+			else
+				leftOld = old[(C - 1)*32 + lane - 1];
+			float run = 0.0f, prevOld = leftOld;
+			for (int c = 0; c < C; ++c)
+				{
+				const float o = old[c*32 + lane];
+				const float b = ADD(prevOld, rowbuf[lane*C + c]);
+				float v = fmaxf(o, b);
+				v = c == 0 ? v : fmaxf(v, run);
+				run = v;
+				pre[c*32 + lane] = v;
+				prevOld = o;
+				}
+			__syncwarp();
+			float scan = run;
+#pragma unroll
+			for (int o = 1; o < 32; o <<= 1)
+				{
+				const float n = __shfl_up_sync(MB_FULL, scan, o);
+				if (lane >= o)
+					scan = fmaxf(scan, n);
+				}
+			float excl = __shfl_up_sync(MB_FULL, scan, 1);
+			const float inc0 = __shfl_sync(MB_FULL, incoming, 0);
+			excl = lane == 0 ? inc0 : fmaxf(excl, inc0);
+			float lastNew = 0.0f;
+			for (int c = 0; c < C; ++c)
+				{
+				lastNew = fmaxf(pre[c*32 + lane], excl);
+				old[c*32 + lane] = lastNew;
+				}
+			if (lane == 31 && !last)
+				eOut[i] = lastNew;
+			__syncwarp();
+			for (uint32_t e0 = 0; e0 < cnt; e0 += 32)
+				{
+				const int idx = (int) cnt - 1 - (int)(e0 + lane);
+				if (idx >= 0)
+					{
+					const int lc = (int) row[idx].col - j0;
+					if (lc >= 0 && lc < W)
+						rowbuf[lc] = 0.0f;
+					}
+				}
+			__syncwarp();
+			}
+		if (strip == 0 && lane == 0)
+			rowoff[LX] = written;
+		if (lane == 31 && !last)
+			eOut[0] = 0.0f;
+		if (last)
+			{
+			// cell (LX,LY), local column g.clast of lane g.lcl.  Which form ptxas compiles best differs by mode:
+			// reading g.clast keeps it live through Backward and costs the plain CM = 14 and 16 kernels a
+			// register and 2 instructions per Backward column; forming the cell from LY instead costs the
+			// MEGA kernels 2 instructions per Backward column.
+			const int q = LY - 1 - j0;
+			eaScore = MEGA ? old[g.clast*32 + g.lcl] : old[(q % C)*32 + q/C];
+			}
+		__syncwarp();
+		float *tmp = eIn; eIn = eOut; eOut = tmp;
+		}
+	if (lane == 0)
+		P.ea[pair] = __fdiv_rn(eaScore, (float) min(LX, LY));     // calcposteriorflat.cpp:89
+	__syncwarp();
 	}
 
 // CM: size class (columns per lane the shared memory is sized for; P.cmax <= CM caps C at run time)
@@ -109,7 +371,6 @@ k_posterior_sm(const PostParams P)
 	float4   *st = reinterpret_cast<float4 *>(wbase);                  // Forward {S, M, IX, JX}; Backward {M, IX, JX, posterior score}
 	uint2    *ye = reinterpret_cast<uint2 *>(wbase + 4*CM*32);         // MEGA only: {letters 0..3, bits of eY}
 	uint32_t *y2 = reinterpret_cast<uint32_t *>(wbase + (MEGA ? 6 : 4)*CM*32);   // MEGA: letters 4..7; plain: class of Y
-	(void) ye;
 
 	mb_logadd_fill(sm.coef, &sm.labase);
 	if (!MEGA)
@@ -151,32 +412,12 @@ k_posterior_sm(const PostParams P)
 		// the work unit is a chain: P.order[chain[w] .. chain[w+1]) are pairs with the same Y, in store order
 		const uint32_t *cpairs = P.order + P.chain[w];
 		const int nch = (int)(P.chain[w + 1] - P.chain[w]);
-		const uint32_t sy = P.py[cpairs[0]];
-		const int LY = (int) P.seqlen[sy];
-		const uint8_t *Yc = P.codes + P.seqoff[sy];
-		const uint2 *Yl = reinterpret_cast<const uint2 *>(P.codes) + P.seqoff[sy];   // MEGA: 8 letter bytes per position
-		const float *Yi = P.insT + P.seqoff[sy];                                     // MEGA: insert emission per position
-		(void) Yc; (void) Yl; (void) Yi;
-		// per-lane pair cursor: the X side of pair k of the chain (loaded once per lane per pair)
-		int LX;
-		const uint8_t *Xc;
-		const uint2 *Xl;
-		const float *Xi;
-		auto load_x = [&](int k)
-			{
-			const uint32_t sx = P.px[cpairs[k]];
-			LX = (int) P.seqlen[sx];
-			Xc = P.codes + P.seqoff[sx];
-			Xl = reinterpret_cast<const uint2 *>(P.codes) + P.seqoff[sx];
-			Xi = P.insT + P.seqoff[sx];
-			};
+		const MbSeq Y = mb_seq(P, P.py[cpairs[0]]);
+		const int LY = Y.len;
 		const int sumLX = __reduce_add_sync(MB_FULL, lane < nch ? P.seqlen[P.px[cpairs[lane]]] : 0u);
 		const int C = min(min(CM, (int) P.cmax), (LY + 31) >> 5);   // columns per lane for this chain
-		const int W = 32*C;
-		const int nstrips = (LY + W - 1)/W;                 // > 1 only for a chain of one pair
-		const int lastj0 = (nstrips - 1)*W;
-		const int lcl = (LY - 1 - lastj0)/C;              // lane / local column of DP column LY
-		const int clast = (LY - 1 - lastj0) - lcl*C;
+		const MbStrips g = mb_strips(LY, C);               // more than one strip only for a chain of one pair
+		const int W = g.W;
 
 		for (int k = 0; k < nch; ++k)
 			ckept[k*32 + lane] = 0;
@@ -186,64 +427,33 @@ k_posterior_sm(const PostParams P)
 		// separator step that resets the lane's state records to LOG_ZERO and passes LOG_ZERO on, so
 		// that row 0 of the next pair sees exactly the border of a fresh pair.  Pair k starts at chain
 		// step Fk + l, Fk = sum over earlier pairs of (LX + 2).
-		for (int strip = 0; strip < nstrips; ++strip)
+		for (int strip = 0; strip < g.n; ++strip)
 			{
-			const int j0 = strip*W;
-			const int ncol = min(W, LY - j0);
-			const int nl = (ncol + C - 1)/C;
-			const bool last = (strip == nstrips - 1);
-			const int cn = (last && lane == lcl) ? clast + 1 : C;     // columns of this lane up to LY
-			const float4 *edgeIn = (strip & 1) ? edge0 : edge1;
-			float4 *edgeOut = (strip & 1) ? edge1 : edge0;
+			const auto [j0, nl, cn, last] = g.at(strip, lane);
+			const auto [edgeIn, edgeOut] = mb_strip_edges(edge0, edge1, strip);
 			float *fms = fm + (size_t) strip*P.fm_rows*W;
 
-			for (int c = 0; c < C; ++c)
-				{
-				const int jj = j0 + lane*C + c;
-				if (MEGA)
-					{
-					const uint2 yl = jj < LY ? Yl[jj] : make_uint2(0u, 0u);
-					ye[c*32 + lane] = make_uint2(yl.x, __float_as_uint(jj < LY ? Yi[jj] : 0.0f));
-					y2[c*32 + lane] = yl.y;
-					}
-				else
-					{
-					const int code = jj < LY ? (int) Yc[jj] : h.pad;
-					y2[c*32 + lane] = (uint32_t) code;
-					}
-				st[c*32 + lane] = make_float4(Z, Z, Z, Z);
-				}
+			mb_stage_y<MEGA>(Y, j0 + lane*C, C, lane, h.pad, st, ye, y2);
 			float outM = Z, outAIY = Z, outAJY = Z, outS = Z;
 			float dprev = Z;
 			float bIX = Z, bJX = Z;
 			const int nsteps = sumLX + 2*nch - 2 + nl;
-			int xcPref = h.pad;
-			uint2 xlPref = make_uint2(0u, 0u);
-			float exPref = 0.0f;
 			int kp = 0, r0 = lane;                // the lane's pair and the step of its row 0
-			load_x(0);
+			MbSeq X = mb_seq(P, P.px[cpairs[0]]);
+			MbXRow xPref = mb_x_row<MEGA>(X, false, 0, h.pad);
 			for (int t = 0; t < nsteps; ++t)
 				{
 				const int i = t - r0;
-				const int xc = xcPref;
-				const uint2 xl = xlPref;
-				const float exm = exPref;
-				if (MEGA)
-					{
-					const bool in = i >= 0 && i < LX;
-					xlPref = in ? Xl[i] : make_uint2(0u, 0u);
-					exPref = in ? Xi[i] : 0.0f;
-					}
-				else
-					xcPref = (i >= 0 && i < LX) ? (int) Xc[i] : h.pad;
-				(void) xc; (void) xl; (void) exm;
+				const MbXRow x = xPref;
+				xPref = mb_x_row<MEGA>(X, i >= 0 && i < X.len, i, h.pad);
 				float Lm = __shfl_up_sync(MB_FULL, outM, 1);
 				float Laiy = __shfl_up_sync(MB_FULL, outAIY, 1);
 				float Lajy = __shfl_up_sync(MB_FULL, outAJY, 1);
 				float Ls = __shfl_up_sync(MB_FULL, outS, 1);
-				if (i >= 0 && i <= LX && lane < nl)
+				if (i >= 0 && i <= X.len && lane < nl)
 					{
-					const float ex = MEGA ? exm : sm.insT[xc];
+					const MbXEmit xe = mb_x_emit<MEGA>(P, sm.insT, meT, h.KS, x);
+					const float ex = xe.ins;
 					if (lane == 0)
 						{
 						if (strip == 0)
@@ -277,36 +487,16 @@ k_posterior_sm(const PostParams P)
 					dprev = Ls;
 					float lm = Lm, laiy = Laiy, lajy = Lajy, sLast = Z;
 					float ix = Z, jx = Z, iy = Z, jy = Z;
-					const float2 *merow = meT + (MEGA ? 0 : xc*h.KS);
-					uint32_t xb[8];
-					if (MEGA)
-						{
-#pragma unroll
-						for (int f = 0; f < 8; ++f)
-							xb[f] = P.mega_base[f] + ((f < 4 ? (xl.x >> (8*f)) : (xl.y >> (8*(f - 4)))) & 255u)*P.mega_alpha[f];
-						}
 					float4 *sp = st + lane;
 					const uint2 *yp = ye + lane;
 					const uint32_t *y2p = y2 + lane;
 					float *dst = fms + (size_t) t*W + lane;
 					const bool dump = DUMP && i >= 1 && cpairs[kp] == P.dbg_pair;
-					(void) y2p; (void) dump;
-MB_UNROLL(MB_SM_UNROLL)
+#pragma unroll 1
 					for (int c = 0; c < cn; ++c, sp += 32, yp += 32, y2p += 32, dst += 32)
 						{
 						const float4 v = *sp;                      // {S, M, IX, JX} of row i-1
-						float em, eyc;
-						if (MEGA)
-							{
-							const uint2 y = *yp;
-							eyc = __uint_as_float(y.y);
-							em = mb_mega_emit(matchT, xb, y.x, *y2p, nf);
-							}
-						else
-							{
-							const float2 e2 = merow[*y2p];
-							em = e2.x; eyc = e2.y;
-							}
+						const auto [em, eyc] = mb_col_emit<MEGA>(matchT, xe, nf, yp, y2p);
 						const float m = ADD(diag, em);
 						ix = ADD(la(ADD(v.z, h.tII), ADD(v.y, h.tMI)), ex);
 						jx = ADD(la(ADD(v.w, h.tJJ), ADD(v.y, h.tMJ)), ex);
@@ -324,7 +514,7 @@ MB_UNROLL(MB_SM_UNROLL)
 						if (dump)
 							P.dbg_fwd[(size_t)(i - 1)*LY + j0 + lane*C + c] = m;
 						}
-					if (last && i == LX && lane == lcl)    // cell (LX,LY) is the lane's last
+					if (last && i == X.len && lane == g.lcl)    // cell (LX,LY) is the lane's last
 						{
 						float *f = cfin + 5*kp;
 						f[0] = lm; f[1] = ix; f[2] = iy; f[3] = jx; f[4] = jy;
@@ -333,16 +523,14 @@ MB_UNROLL(MB_SM_UNROLL)
 					if (lane == 31 && !last)
 						edgeOut[i] = make_float4(outM, outAIY, outAJY, outS);
 					}
-				else if (i == LX + 1 && lane < nl)        // separator, then the next pair of the chain
+				else if (i == X.len + 1 && lane < nl)        // separator, then the next pair of the chain
 					{
-#pragma unroll 1
-					for (int c = 0; c < C; ++c)
-						st[c*32 + lane] = make_float4(Z, Z, Z, Z);
+					mb_clear_state(st, C, lane);
 					outM = Z; outAIY = Z; outAJY = Z; outS = Z;
 					dprev = Z;
 					if (++kp < nch)
 						{
-						load_x(kp);
+						X = mb_seq(P, P.px[cpairs[kp]]);
 						r0 = t + 1;
 						}
 					else
@@ -387,65 +575,33 @@ MB_UNROLL(MB_SM_UNROLL)
 		const float keepScore = fmaxf(h.minScore, __uint_as_float(0xc0935d8eu));
 		uint32_t kept = 0;
 		bool overflow = false;
-		for (int strip = nstrips - 1; strip >= 0; --strip)
+		for (int strip = g.n - 1; strip >= 0; --strip)
 			{
-			const int j0 = strip*W;
-			const int ncol = min(W, LY - j0);
-			const int nl = (ncol + C - 1)/C;
-			const bool last = (strip == nstrips - 1);
-			const int cn = (last && lane == lcl) ? clast + 1 : C;     // columns of this lane up to LY
-			const float4 *edgeIn = (strip & 1) ? edge0 : edge1;
-			float4 *edgeOut = (strip & 1) ? edge1 : edge0;
+			const auto [j0, nl, cn, last] = g.at(strip, lane);
+			const auto [edgeIn, edgeOut] = mb_strip_edges(edge0, edge1, strip);
 			const float *fms = fm + (size_t) strip*P.fm_rows*W;
 
-			for (int c = 0; c < C; ++c)
-				{
-				const int jj = j0 + lane*C + c + 1;
-				if (MEGA)
-					{
-					const uint2 yl = jj < LY ? Yl[jj] : make_uint2(0u, 0u);
-					ye[c*32 + lane] = make_uint2(yl.x, __float_as_uint(jj < LY ? Yi[jj] : 0.0f));
-					y2[c*32 + lane] = yl.y;
-					}
-				else
-					{
-					const int code = jj < LY ? (int) Yc[jj] : h.pad;
-					y2[c*32 + lane] = (uint32_t) code;
-					}
-				st[c*32 + lane] = make_float4(Z, Z, Z, Z);
-				}
+			mb_stage_y<MEGA>(Y, j0 + lane*C + 1, C, lane, h.pad, st, ye, y2);
 			float outM = Z, outIY = Z, outJY = Z;
 			uint32_t outCnt = 0;
 			float dprev = Z;
 			const int nsteps = sumLX + nch - 2 + nl;
-			int xcPref = h.pad;
-			uint2 xlPref = make_uint2(0u, 0u);
-			float exPref = 0.0f;
 			int kp = nch - 1, u0 = nl - 1 - lane;   // the lane's pair and the step of its row LX
-			load_x(nch - 1);
-			int fk = sumLX - LX + 2*(nch - 1);      // chain Forward step of the pair's row 0, less the lane
-			int rk = sumLX - LX;                  // chain row of the pair's row 1 in rows / rowcnt
+			MbSeq X = mb_seq(P, P.px[cpairs[nch - 1]]);
+			MbXRow xPref = mb_x_row<MEGA>(X, false, 0, h.pad);
+			int fk = sumLX - X.len + 2*(nch - 1);   // chain Forward step of the pair's row 0, less the lane
+			int rk = sumLX - X.len;               // chain row of the pair's row 1 in rows / rowcnt
 			float total = ctotal[nch - 1];
 			for (int u = 0; u < nsteps; ++u)
 				{
-				const int i = LX - u + u0;
-				const int xc = xcPref;
-				const uint2 xl = xlPref;
-				const float exm = exPref;
-				if (MEGA)
-					{
-					const bool in = i >= 2 && i <= LX;
-					xlPref = in ? Xl[i - 1] : make_uint2(0u, 0u);
-					exPref = in ? Xi[i - 1] : 0.0f;
-					}
-				else
-					xcPref = (i >= 2 && i <= LX) ? (int) Xc[i - 1] : h.pad;
-				(void) xc; (void) xl; (void) exm;
+				const int i = X.len - u + u0;
+				const MbXRow x = xPref;
+				xPref = mb_x_row<MEGA>(X, i >= 2 && i <= X.len, i - 1, h.pad);
 				float Rm = __shfl_down_sync(MB_FULL, outM, 1);
 				float Riy = __shfl_down_sync(MB_FULL, outIY, 1);
 				float Rjy = __shfl_down_sync(MB_FULL, outJY, 1);
 				uint32_t cnt = __shfl_down_sync(MB_FULL, outCnt, 1);    // entries already in the row
-				if (i >= 1 && i <= LX && lane < nl)
+				if (i >= 1 && i <= X.len && lane < nl)
 					{
 					if (lane == nl - 1)
 						{
@@ -459,15 +615,8 @@ MB_UNROLL(MB_SM_UNROLL)
 							Rm = e.x; Riy = e.y; Rjy = e.z; cnt = __float_as_uint(e.w);
 							}
 						}
-					const float ex = MEGA ? exm : sm.insT[xc];
-					const float2 *merow = meT + (MEGA ? 0 : xc*h.KS);
-					uint32_t xb[8];
-					if (MEGA)
-						{
-#pragma unroll
-						for (int f = 0; f < 8; ++f)
-							xb[f] = P.mega_base[f] + ((f < 4 ? (xl.x >> (8*f)) : (xl.y >> (8*(f - 4)))) & 255u)*P.mega_alpha[f];
-						}
+					const MbXEmit xe = mb_x_emit<MEGA>(P, sm.insT, meT, h.KS, x);
+					const float ex = xe.ins;
 					const int t = fk + i + lane;
 					const int col0 = j0 + lane*C;
 					float mdiag = dprev;
@@ -492,10 +641,9 @@ MB_UNROLL(MB_SM_UNROLL)
 					const uint2 *yp = ye + lane;
 					const uint32_t *y2p = y2 + lane;
 					const float *src = fms + (size_t) t*W + lane;     // Forward M of the lane's column 0
-					(void) y2p;
 					int c = cn - 1;
 					sp += c*32; yp += c*32; y2p += c*32; src += c*32;
-					if (last && i == LX && lane == lcl)
+					if (last && i == X.len && lane == g.lcl)
 						{
 						// cell (LX,LY), the lane's first: the end scores (bwdflat3.cpp:53-61)
 						mdiag = sp->x;
@@ -510,7 +658,7 @@ MB_UNROLL(MB_SM_UNROLL)
 					// step t-1's column C-1 (t is the same in every lane), inside this warp's spill since t >= 1
 					float fmNext = *src;                       // column c
 					float fmNext2 = c >= 1 ? src[-32] : 0.0f;  // column c-1
-MB_UNROLL(MB_SM_UNROLL)
+#pragma unroll 1
 					for (; c >= 0; --c, sp -= 32, yp -= 32, y2p -= 32)
 						{
 						const float fmv = fmNext;
@@ -519,18 +667,7 @@ MB_UNROLL(MB_SM_UNROLL)
 						if (c >= 2)
 							fmNext2 = src[-32];                // column c-2
 						const float4 v = *sp;                      // {M, IX, JX, score} of row i+1
-						float em, eyc;
-						if (MEGA)
-							{
-							const uint2 y = *yp;
-							eyc = __uint_as_float(y.y);
-							em = mb_mega_emit(matchT, xb, y.x, *y2p, nf);
-							}
-						else
-							{
-							const float2 e2 = merow[*y2p];
-							em = e2.x; eyc = e2.y;
-							}
+						const auto [em, eyc] = mb_col_emit<MEGA>(matchT, xe, nf, yp, y2p);
 						const float nM = ADD(mdiag, em);
 						const float nIX = ADD(v.y, ex);
 						const float nJX = ADD(v.z, ex);
@@ -574,19 +711,17 @@ MB_UNROLL(MB_SM_UNROLL)
 					}
 				else if (i == 0 && lane < nl)         // separator, then the previous pair of the chain
 					{
-#pragma unroll 1
-					for (int c = 0; c < C; ++c)
-						st[c*32 + lane] = make_float4(Z, Z, Z, Z);
+					mb_clear_state(st, C, lane);
 					outM = Z; outIY = Z; outJY = Z;
 					outCnt = 0;
 					dprev = Z;
 					ckept[kp*32 + lane] = kept;
 					if (kp > 0)
 						{
-						load_x(--kp);
+						X = mb_seq(P, P.px[cpairs[--kp]]);
 						u0 = u + 1;
-						fk -= LX + 2;
-						rk -= LX;
+						fk -= X.len + 2;
+						rk -= X.len;
 						total = ctotal[kp];
 						}
 					else
@@ -603,145 +738,14 @@ MB_UNROLL(MB_SM_UNROLL)
 
 		// ============================ compaction + expected accuracy, pair by pair ============================
 		int rk = 0;
-		for (int k = 0; k < nch; rk += LX, ++k)
+		for (int k = 0; k < nch; ++k)
 			{
 			const uint32_t pair = cpairs[k];
-			LX = (int) P.seqlen[P.px[pair]];
-			uint32_t kept = ckept[k*32 + lane] - (k + 1 < nch ? ckept[(k + 1)*32 + lane] : 0u);
-			for (int o = 16; o > 0; o >>= 1)
-				kept += __shfl_xor_sync(MB_FULL, kept, o);
-			unsigned long long base = 0;
-			if (lane == 0)
-				base = atomicAdd(P.ent_cursor, (unsigned long long) kept);
-			base = __shfl_sync(MB_FULL, base, 0);
-			const bool fits = (base + kept <= P.ent_cap);
-			if (lane == 0)
-				{
-				if (!fits)
-					atomicCAS(P.err, 0, MB200_ENOMEM);
-				P.entbase[pair] = base;
-				P.nnz[pair] = kept;
-				}
-			const mb200_entry *prow = rows + (size_t) rk*MB_CAP;
-			const uint8_t *pcnt = rowcnt + rk;
-			uint32_t *rowoff = P.rowoff + P.rowbase[pair];
-			mb200_entry *out = P.entries + base;
-
-			float eaScore = 0.0f;
-			{
-			// the warp's state area, reused as three plain float arrays of CM*32
-			float *old = wbase;                 // [c][lane]
-			float *rowbuf = wbase + CM*32;      // column-linear: [lane*C + c]
-			float *pre = wbase + 2*CM*32;       // [c][lane]
-			float *eIn = reinterpret_cast<float *>(edge0);
-			float *eOut = reinterpret_cast<float *>(edge1);
-			uint32_t written = 0;
-			for (int strip = 0; strip < nstrips; ++strip)
-				{
-				const int j0 = strip*W;
-				for (int c = 0; c < C; ++c)
-					{
-					old[c*32 + lane] = 0.0f;
-					rowbuf[c*32 + lane] = 0.0f;
-					}
-				__syncwarp();
-				for (int i = 1; i <= LX; ++i)
-					{
-					const uint32_t cnt = pcnt[i - 1];
-					const mb200_entry *row = prow + (size_t)(i - 1)*MB_CAP;
-					if (strip == 0 && lane == 0)
-						rowoff[i - 1] = written;
-					for (uint32_t e0 = 0; e0 < cnt; e0 += 32)
-						{
-						const int idx = (int) cnt - 1 - (int)(e0 + lane);
-						mb200_entry ent; ent.p = 0.0f; ent.col = 0;
-						if (idx >= 0)
-							{
-							ent = row[idx];             // {score, column}: the probability (calcposteriorflat.cpp:20)
-							ent.p = ent.p >= 0.0f ? 1.0f : mb_expf_glibc(ent.p);
-							}
-						const int lc = (int) ent.col - j0;
-						if (idx >= 0 && lc >= 0 && lc < W)
-							rowbuf[lc] = ent.p;
-						if (strip == 0)
-							{
-							const bool keep = idx >= 0 && ent.p >= 0.01f;          // mysparsemx.cpp:139-141
-							const uint32_t b = __ballot_sync(MB_FULL, keep);
-							if (keep && fits)
-								out[written + __popc(b & ((1u << lane) - 1u))] = ent;
-							written += __popc(b);
-							}
-						}
-					__syncwarp();
-					// calcalnscoreflat.cpp:13-29 as a prefix-max over the row
-					float leftOld = 0.0f, incoming = 0.0f;
-					if (lane == 0)
-						{
-						leftOld = strip == 0 ? 0.0f : eIn[i - 1];
-						incoming = strip == 0 ? 0.0f : eIn[i];
-						}
-					else
-						leftOld = old[(C - 1)*32 + lane - 1];
-					float run = 0.0f, prevOld = leftOld;
-					for (int c = 0; c < C; ++c)
-						{
-						const float o = old[c*32 + lane];
-						const float b = ADD(prevOld, rowbuf[lane*C + c]);
-						float v = fmaxf(o, b);
-						v = c == 0 ? v : fmaxf(v, run);
-						run = v;
-						pre[c*32 + lane] = v;
-						prevOld = o;
-						}
-					__syncwarp();
-					float scan = run;
-#pragma unroll
-					for (int o = 1; o < 32; o <<= 1)
-						{
-						const float n = __shfl_up_sync(MB_FULL, scan, o);
-						if (lane >= o)
-							scan = fmaxf(scan, n);
-						}
-					float excl = __shfl_up_sync(MB_FULL, scan, 1);
-					const float inc0 = __shfl_sync(MB_FULL, incoming, 0);
-					excl = lane == 0 ? inc0 : fmaxf(excl, inc0);
-					float lastNew = 0.0f;
-					for (int c = 0; c < C; ++c)
-						{
-						lastNew = fmaxf(pre[c*32 + lane], excl);
-						old[c*32 + lane] = lastNew;
-						}
-					if (lane == 31 && strip + 1 < nstrips)
-						eOut[i] = lastNew;
-					__syncwarp();
-					for (uint32_t e0 = 0; e0 < cnt; e0 += 32)
-						{
-						const int idx = (int) cnt - 1 - (int)(e0 + lane);
-						if (idx >= 0)
-							{
-							const int lc = (int) row[idx].col - j0;
-							if (lc >= 0 && lc < W)
-								rowbuf[lc] = 0.0f;
-							}
-						}
-					__syncwarp();
-					}
-				if (strip == 0 && lane == 0)
-					rowoff[LX] = written;
-				if (lane == 31 && strip + 1 < nstrips)
-					eOut[0] = 0.0f;
-				if (strip == nstrips - 1)
-					{
-					const int q = LY - 1 - j0;          // column-local index of DP column LY
-					eaScore = old[(q % C)*32 + q/C];
-					}
-				__syncwarp();
-				float *tmp = eIn; eIn = eOut; eOut = tmp;
-				}
-			}
-			if (lane == 0)
-				P.ea[pair] = __fdiv_rn(eaScore, (float) min(LX, LY));     // calcposteriorflat.cpp:89
-			__syncwarp();
+			const int LX = (int) P.seqlen[P.px[pair]];
+			mb_compact_ea<MEGA, CM>(P, pair, LX, LY, ckept[k*32 + lane] - (k + 1 < nch ? ckept[(k + 1)*32 + lane] : 0u),
+			  rows + (size_t) rk*MB_CAP, rowcnt + rk, g, wbase, reinterpret_cast<float *>(edge0),
+			  reinterpret_cast<float *>(edge1));
+			rk += LX;
 			}
 		}
 	}
