@@ -36,12 +36,6 @@
 #include <cstdlib>
 #include <cstring>
 
-#define CU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) \
-	return mb_fail(ctx, e_ == cudaErrorMemoryAllocation ? MB200_ENOMEM : MB200_ECUDA, \
-	  "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
-#define ENSURE(buf, bytes) do { if ((buf).ensure(bytes) != 0) \
-	return mb_fail(ctx, MB200_ENOMEM, "device allocation of %zu bytes failed (%s)", (size_t)(bytes), #buf); } while (0)
-
 // MB200_TRACE=1: wall-time split of the join path, printed at process exit
 static bool g_trace = false;
 static int g_trace_level = 0;          // 2: one line per join of >= 64 sequences
@@ -60,8 +54,6 @@ static void trace_report()
 		fprintf(stderr, "[mb200 trace] BuildPost by cell: count+order %.2f s, emit %.2f s, sort %.2f s, runs %.2f s, sum %.2f s\n",
 		  g_ts[0], g_ts[1], g_ts[2], g_ts[3], g_ts[4]);
 	}
-#define TRACE_SUB(k) do { if (g_trace) { cudaStreamSynchronize(st); const double n_ = now_s(); g_ts[k] += n_ - tsub; tsub = n_; } } while (0)
-#define TRACE_MARK(k) do { if (g_trace) { cudaStreamSynchronize(st); const double n_ = now_s(); g_t[k] += n_ - tmark; tmark = n_; } } while (0)
 static void trace_init()
 	{
 	static bool done = false;
@@ -75,6 +67,16 @@ static void trace_init()
 		atexit(trace_report);
 		}
 	}
+// The running marks of one join: mark(k) adds the time since the previous mark to g_t[k], sub(k) the
+// time since the previous sub to g_ts[k].  Both synchronise the stream, and only when tracing.
+struct JoinTimer
+	{
+	cudaStream_t st;
+	double tmark, tsub = 0;
+	explicit JoinTimer(cudaStream_t s) : st(s) { trace_init(); tmark = now_s(); ++g_calls; }
+	void mark(int k) { if (g_trace) { cudaStreamSynchronize(st); const double n = now_s(); g_t[k] += n - tmark; tmark = n; } }
+	void sub(int k) { if (g_trace) { cudaStreamSynchronize(st); const double n = now_s(); g_ts[k] += n - tsub; tsub = n; } }
+	};
 
 // =============================================================================================
 // decoding DP
@@ -1130,225 +1132,284 @@ __global__ void k_iota(uint32_t n, uint32_t *__restrict__ out)
 // =============================================================================================
 // host side
 static inline size_t al256(size_t b) { return (b + 255)/256*256; }
-static inline size_t aw_dense_bytes(size_t LX, size_t ld) { return (LX + 1 + AW_PAD_BOT)*ld*sizeof(float); }
 
-struct JoinBufs                       // carved out of ctx->d_join
+// Geometry of one k_aln_wave problem (LX rows, LY columns) and the bytes of its pieces.  Every size is
+// non-decreasing in LX and LY, and tb_smem can only turn on as they shrink.
+struct AlnLayout
 	{
-	float *post; uint32_t ld;
-	uint8_t *tb; uint2 *edge; char *path; float *score; uint32_t *plen; AlnProblem *prob;
+	uint32_t LX, LY, ld, nstrips, nwarps, npass;
+	bool tb_smem;                    // one CTA keeps the traceback in shared memory (tb_bytes of it)
+	size_t dense_bytes;              // the matrix with its zero row above and AW_PAD_BOT rows below
+	size_t tb_bytes;                 // traceback [LX][nstrips*32]
+	size_t chan_bytes;               // hand-over channel [npass][LX+1], the done word in its last 256 bytes
+	size_t path_bytes;
+	size_t tb_carve() const { return tb_smem ? 256 : al256(tb_bytes); }
+	// one problem as join_core carves it: dense | tb | channel | path | score | plen | the AlnProblem
+	size_t bytes() const { return al256(dense_bytes) + tb_carve() + chan_bytes + al256(path_bytes) + 3*256; }
 	};
-
-// BuildPost + decoding DP of groups whose maps are already on the device.  Leaves path / plen /
-// score on the device (JoinBufs) and does NOT synchronise.
-static int join_core(mb200_ctx *ctx, uint32_t na, uint32_t nb, const uint32_t *d_ida, const uint32_t *d_idb,
-  const int32_t *d_c2pa, const uint32_t *d_p2cb, const uint64_t *d_boff, const uint32_t *d_rb, const std::vector<uint32_t> &h_rb,
-  uint32_t cols_a, uint32_t cols_b, char *scratch, size_t scratch_bytes, JoinBufs &B, double &tmark)
+static AlnLayout aln_layout(uint32_t LX, uint32_t LY, bool smem_ok)
 	{
-	cudaStream_t st = ctx->stream;
-	const uint32_t ld = (cols_b + AW_C - 1)/AW_C*AW_C;
-	const uint32_t nstrips = (cols_b + AW_W - 1)/AW_W;
-	const size_t post_bytes = aw_dense_bytes(cols_a, ld);         // incl. the zero row above and the padding below
-	const uint32_t nwarps = std::min<uint32_t>(AW_MAXW, nstrips);
-	const uint32_t npass = (nstrips + nwarps - 1)/nwarps;
-	const size_t tbw = (size_t) cols_a*nstrips*32;
-	const bool tb_smem = npass == 1 && tbw <= 192*1024;
-	const size_t chan_bytes = al256((size_t) npass*((size_t) cols_a + 1)*sizeof(uint2) + 256);
-	char *p = scratch;
-	B.post = (float *) p + ld;       p += al256(post_bytes);
-	B.tb = (uint8_t *) p;            p += tb_smem ? 256 : al256(tbw);
-	B.edge = (uint2 *) p;            p += chan_bytes;
-	B.path = p;                      p += al256((size_t) cols_a + cols_b + 16);
-	B.score = (float *) p;           p += 256;
-	B.plen = (uint32_t *) p;         p += 256;
-	B.prob = (AlnProblem *) p;       p += 256;
-	B.ld = ld;
-	if ((size_t)(p - scratch) > scratch_bytes)
-		return mb_fail(ctx, MB200_EINVAL, "join scratch too small");
-	CU(cudaMemsetAsync(B.post - ld, 0, post_bytes, st));
-
-	BuildPostParams P;
-	P.n = ctx->nseq; P.na = na; P.nb = nb; P.cols_a = cols_a; P.cols_b = cols_b; P.ld = ld;
-	P.ids_a = d_ida; P.ids_b = d_idb; P.col2pos_a = d_c2pa; P.p2c_b = d_p2cb; P.p2c_b_off = d_boff;
-	P.rowbase = (const uint64_t *) ctx->d_rowbase.p; P.rowoff = (const uint32_t *) ctx->d_rowoff.p;
-	P.entries = (const mb200_entry *) ctx->d_entries.p;
-	P.trbase = (const uint64_t *) ctx->d_tr_rowbase.p; P.troff = (const uint32_t *) ctx->d_tr_rowoff.p;
-	P.trentries = (const mb200_entry *) ctx->d_tr_entries.p;
-	P.entbase = (const uint64_t *) ctx->d_entbase.p;
-	P.post = B.post;
-	// large joins: bucket the contributions by cell (see k_bpc_*); small ones: ordered row walk (k_bp_apply)
-	size_t nbatches = 0;
-	const char *ev_sort = getenv("MB200_BP_SORT_MIN");             // tuning hook: (residues of A) x |B| from which to sort
-	const long long sort_min = ev_sort ? atoll(ev_sort) : 1000000ll;
-	uint32_t colbits = 1, rowbits = 1;
-	while ((1u << colbits) < cols_b)
-		++colbits;
-	while ((1u << rowbits) < cols_a)
-		++rowbits;
-	if ((uint64_t) h_rb[na]*nb >= (uint64_t) sort_min && colbits + rowbits <= 32 && na <= 65535)
+	AlnLayout L;
+	L.LX = LX; L.LY = LY;
+	L.ld = (LY + AW_C - 1)/AW_C*AW_C;
+	L.nstrips = (LY + AW_W - 1)/AW_W;
+	L.nwarps = std::min<uint32_t>(AW_MAXW, L.nstrips);
+	L.npass = (L.nstrips + L.nwarps - 1)/L.nwarps;
+	L.tb_bytes = (size_t) LX*L.nstrips*32;
+	L.tb_smem = smem_ok && L.npass == 1 && L.tb_bytes <= 192*1024;
+	L.dense_bytes = ((size_t) LX + 1 + AW_PAD_BOT)*L.ld*sizeof(float);
+	L.chan_bytes = al256((size_t) L.npass*((size_t) LX + 1)*sizeof(uint2) + 256);
+	L.path_bytes = (size_t) LX + LY + 16;
+	return L;
+	}
+static void aln_place(const AlnLayout &L, char *dense, char *tb, char *chan, char *path, AlnProblem &q)
+	{
+	q.LX = L.LX; q.LY = L.LY; q.ld = L.ld;
+	q.dense = (const float *) dense + L.ld;
+	q.tb = (uint8_t *) tb;
+	q.edge = (uint2 *) chan;
+	q.done = (uint32_t *)(chan + L.chan_bytes - 256);
+	q.path = path;
+	}
+// A join's members, A then B, and their copies at the front of ctx->d_join: ids, rb [na+1] (A's residues before
+// member s), boff [nb] (B's member t in the concatenated pos->col maps), c2p [na][c2p cols], p2cb [btot]
+struct JoinMembers
+	{
+	uint32_t na = 0, nb = 0, lmax = 0;
+	uint64_t btot = 0;
+	std::vector<uint32_t> ids, h_rb;
+	std::vector<uint64_t> boff;
+	uint32_t *d_ids = nullptr, *d_rb = nullptr, *d_p2cb = nullptr;
+	uint64_t *d_boff = nullptr;
+	int32_t *d_c2p = nullptr;
+	};
+// Checks the store and that every id is in range and listed once (A and B disjoint); builds the host maps
+static int join_members(mb200_ctx *ctx, const char *who, uint32_t na, const uint32_t *ids_a, uint32_t nb, const uint32_t *ids_b,
+  JoinMembers &M)
+	{
+	if (!ctx->store_valid || !ctx->store_allpairs)
+		return mb_fail(ctx, MB200_EINVAL, "%s: the store must hold all N(N-1)/2 pairs", who);
+	int rc = mb_store_build_transposed(ctx);
+	if (rc != MB200_OK)
+		return rc;
+	if (ctx->tr_values_stale)
 		{
-		// batches of sequences of A: at most ~16M (residue, t) rows each
-		const uint64_t budget_rt = 16ull << 20;
-		std::vector<uint32_t> cuts(1, 0);
-		uint64_t max_rt = 0;
-		uint32_t max_res = 0;
-		for (uint32_t s0 = 0; s0 < na; )
+		rc = mb_store_refresh_transposed(ctx);
+		if (rc != MB200_OK)
+			return rc;
+		ctx->tr_values_stale = false;
+		}
+	M.na = na; M.nb = nb;
+	M.ids.resize(na + nb);
+	M.h_rb.assign(na + 1, 0);
+	M.boff.resize(nb);
+	std::vector<uint8_t> member(ctx->nseq, 0);
+	for (uint32_t m = 0; m < na + nb; ++m)
+		{
+		const uint32_t s = m < na ? ids_a[m] : ids_b[m - na];
+		if (s >= ctx->nseq || member[s])
+			return mb_fail(ctx, MB200_EINVAL, "%s: sequence id %u out of range, listed twice, or in both groups "
+			  "(the reference asserts SMI_1 != SMI_2, buildpostflat.cpp:49)", who, s);
+		member[s] = 1;
+		M.ids[m] = s;
+		M.lmax = std::max(M.lmax, ctx->h_len[s]);
+		if (m < na)
+			M.h_rb[m + 1] = M.h_rb[m] + ctx->h_len[s];
+		else
 			{
-			uint32_t e = s0 + 1;
-			while (e < na && (uint64_t)(h_rb[e + 1] - h_rb[s0])*nb <= budget_rt)
-				++e;
-			max_rt = std::max<uint64_t>(max_rt, (uint64_t)(h_rb[e] - h_rb[s0])*nb);
-			max_res = std::max(max_res, h_rb[e] - h_rb[s0]);
-			cuts.push_back(e);
-			s0 = e;
-			}
-		if (max_rt >= 0x7ffffff0ull)
-			return mb_fail(ctx, MB200_EOVERFLOW, "BuildPost batch of %llu rows", (unsigned long long) max_rt);
-		// d_tmp: rowof, seqof [residues] | cnt [max_rt+1] | off [max_rt+1] | eptr [max_rt] | 5 x [max_res] | nruns | cub scratch
-		const size_t rowof_b = al256((size_t) h_rb[na]*4), rt_b = al256((size_t)(max_rt + 1)*4), res_b = al256((size_t) max_res*4);
-		size_t scan_tb = 0, rsort_tb = 0;
-		cub::DeviceScan::ExclusiveSum(nullptr, scan_tb, (const uint32_t *) nullptr, (uint32_t *) nullptr, (int)(max_rt + 1), st);
-		cub::DeviceRadixSort::SortPairs(nullptr, rsort_tb, (const uint32_t *) nullptr, (uint32_t *) nullptr,
-		  (const uint32_t *) nullptr, (uint32_t *) nullptr, (int) max_res, 0, (int) rowbits, st);
-		const size_t tb1 = al256(std::max(scan_tb, rsort_tb));
-		ENSURE(ctx->d_tmp, 2*rowof_b + 4*rt_b + 5*res_b + 256 + tb1);
-		char *tp = (char *) ctx->d_tmp.p;
-		uint32_t *d_rowof = (uint32_t *) tp;             tp += rowof_b;
-		uint32_t *d_seqof = (uint32_t *) tp;             tp += rowof_b;
-		uint64_t *d_eptr = (uint64_t *) tp;              tp += 2*rt_b;
-		uint32_t *d_cnt = (uint32_t *) tp;               tp += rt_b;
-		uint32_t *d_off = (uint32_t *) tp;               tp += rt_b;
-		uint32_t *d_rk = (uint32_t *) tp;                tp += res_b;      // row of the residue / sorted
-		uint32_t *d_ri = (uint32_t *) tp;                tp += res_b;      // local index
-		uint32_t *d_rk2 = (uint32_t *) tp;               tp += res_b;
-		uint32_t *d_perm = (uint32_t *) tp;              tp += res_b;      // residues in (row, s) order
-		uint32_t *d_base = (uint32_t *) tp;              tp += res_b;
-		uint32_t *d_nruns = (uint32_t *) tp;             tp += 256;
-		void *d_scratch1 = tp;
-		k_bp_rowof<<<dim3((cols_a + 255)/256, na), 256, 0, st>>>(P, d_rb, d_rowof, d_seqof);
-		CU(cudaGetLastError());
-		const int sms = ctx->prop.multiProcessorCount;
-		nbatches = cuts.size() - 1;
-		for (size_t b = 0; b + 1 < cuts.size(); ++b)
-			{
-			double tsub = now_s();
-			BpCells C;
-			C.s_lo = cuts[b]; C.s_n = cuts[b + 1] - cuts[b];
-			C.rb = d_rb; C.rowof = d_rowof; C.seqof = d_seqof; C.cnt = d_cnt; C.eptr = d_eptr; C.off = d_off; C.base = d_base;
-			C.colbits = colbits;
-			C.keys = nullptr; C.vals = nullptr;
-			const uint32_t nres = h_rb[cuts[b + 1]] - h_rb[cuts[b]];
-			const uint64_t rt = (uint64_t) nres*nb;
-			const uint32_t gblocks = (uint32_t) std::min<uint64_t>((rt + 255)/256, (uint64_t) sms*32);
-			const uint32_t rblocks = (nres + 255)/256;
-			k_bpc_count<<<gblocks, 256, 0, st>>>(P, C);
-			CU(cudaMemsetAsync(d_cnt + rt, 0, 4, st));
-			size_t t0 = tb1;
-			cub::DeviceScan::ExclusiveSum(d_scratch1, t0, (const uint32_t *) d_cnt, d_off, (int)(rt + 1), st);
-			CU(cudaGetLastError());
-			CU(cudaMemcpyAsync(ctx->h_pinned + 4, d_off + rt, 4, cudaMemcpyDeviceToHost, st));
-			// residues ordered by (row, s): the input order is s-major, the sort is stable
-			k_bpc_reskeys<<<rblocks, 256, 0, st>>>(nres, d_rowof + h_rb[cuts[b]], d_rk, d_ri);
-			t0 = tb1;
-			cub::DeviceRadixSort::SortPairs(d_scratch1, t0, (const uint32_t *) d_rk, d_rk2, (const uint32_t *) d_ri, d_perm,
-			  (int) nres, 0, (int) rowbits, st);
-			k_bpc_resterms<<<rblocks, 256, 0, st>>>(nres, nb, d_perm, d_off, d_rk);           // d_rk: terms per residue, sorted order
-			t0 = tb1;
-			cub::DeviceScan::ExclusiveSum(d_scratch1, t0, (const uint32_t *) d_rk, d_rk2, (int) nres, st);
-			k_bpc_resbase<<<rblocks, 256, 0, st>>>(nres, d_perm, d_rk2, d_base);
-			CU(cudaGetLastError());
-			CU(cudaStreamSynchronize(st));
-			const uint64_t M = ctx->h_pinned[4];
-			if (M >= 0x7fffffffull)
-				return mb_fail(ctx, MB200_EOVERFLOW, "BuildPost batch of %llu terms", (unsigned long long) M);
-			if (M == 0)
-				continue;
-			// d_stage: keys_in | vals_in | keys_out | vals_out | run offsets | cub scratch
-			const size_t mb = al256((size_t) M*4);
-			size_t sort_tb = 0, rle_tb = 0, scan2_tb = 0;
-			cub::DeviceRadixSort::SortPairs(nullptr, sort_tb, (const uint32_t *) nullptr, (uint32_t *) nullptr,
-			  (const float *) nullptr, (float *) nullptr, (int) M, 0, (int) colbits, st);
-			cub::DeviceRunLengthEncode::Encode(nullptr, rle_tb, (const uint32_t *) nullptr, (uint32_t *) nullptr, (uint32_t *) nullptr,
-			  (uint32_t *) nullptr, (int) M, st);
-			cub::DeviceScan::ExclusiveSum(nullptr, scan2_tb, (const uint32_t *) nullptr, (uint32_t *) nullptr, (int) M, st);
-			const size_t tb = std::max(sort_tb, std::max(rle_tb, scan2_tb));
-			ENSURE(ctx->d_stage, 5*mb + al256(tb) + 256);
-			char *sp = (char *) ctx->d_stage.p;
-			uint32_t *keys_in = (uint32_t *) sp;              float *vals_in = (float *)(sp + mb);
-			uint32_t *keys_out = (uint32_t *)(sp + 2*mb);     float *vals_out = (float *)(sp + 3*mb);
-			uint32_t *uoff = (uint32_t *)(sp + 4*mb);
-			void *scratch2 = sp + 5*mb;
-			C.keys = keys_in; C.vals = vals_in;
-			TRACE_SUB(0);
-			k_bpc_emit<<<(uint32_t) std::min<uint64_t>((rt*8 + 255)/256, (uint64_t) sms*32), 256, 0, st>>>(P, C);
-			CU(cudaGetLastError());
-			TRACE_SUB(1);
-			TRACE_MARK(1);
-			// stable sort on the column bits only: (row, s, t) order survives inside every column
-			size_t t1 = sort_tb;
-			cub::DeviceRadixSort::SortPairs(scratch2, t1, (const uint32_t *) keys_in, keys_out, (const float *) vals_in, vals_out,
-			  (int) M, 0, (int) colbits, st);
-			TRACE_SUB(2);
-			// runs of equal cells: unique keys and lengths reuse the input buffers
-			uint32_t *ukeys = keys_in, *ucnt = (uint32_t *) vals_in;
-			size_t t2 = rle_tb;
-			cub::DeviceRunLengthEncode::Encode(scratch2, t2, (const uint32_t *) keys_out, ukeys, ucnt, d_nruns, (int) M, st);
-			CU(cudaGetLastError());
-			CU(cudaMemcpyAsync(ctx->h_pinned + 4, d_nruns, 4, cudaMemcpyDeviceToHost, st));
-			CU(cudaStreamSynchronize(st));
-			const uint32_t nruns = ctx->h_pinned[4];
-			size_t t3 = scan2_tb;
-			cub::DeviceScan::ExclusiveSum(scratch2, t3, (const uint32_t *) ucnt, uoff, (int) nruns, st);
-			// runs by descending length (d_tmp2: counts out | index in | index out | cub scratch)
-			size_t lsort_tb = 0;
-			cub::DeviceRadixSort::SortPairsDescending(nullptr, lsort_tb, (const uint32_t *) nullptr, (uint32_t *) nullptr,
-			  (const uint32_t *) nullptr, (uint32_t *) nullptr, (int) nruns, 0, 32, st);
-			const size_t nrb = al256((size_t) nruns*4);
-			ENSURE(ctx->d_tmp2, 3*nrb + al256(lsort_tb));
-			uint32_t *d_lc = (uint32_t *) ctx->d_tmp2.p;
-			uint32_t *d_li = (uint32_t *)((char *) ctx->d_tmp2.p + nrb);
-			uint32_t *d_lperm = (uint32_t *)((char *) ctx->d_tmp2.p + 2*nrb);
-			void *d_lscratch = (char *) ctx->d_tmp2.p + 3*nrb;
-			k_iota<<<(nruns + 255)/256, 256, 0, st>>>(nruns, d_li);
-			cub::DeviceRadixSort::SortPairsDescending(d_lscratch, lsort_tb, (const uint32_t *) ucnt, d_lc, (const uint32_t *) d_li, d_lperm,
-			  (int) nruns, 0, 32, st);
-			k_count_ge<<<1, 1, 0, st>>>(d_lc, nruns, BPC_LONG, d_nruns + 1);
-			CU(cudaMemcpyAsync(ctx->h_pinned + 5, d_nruns + 1, 4, cudaMemcpyDeviceToHost, st));
-			CU(cudaStreamSynchronize(st));
-			const uint32_t nlong = ctx->h_pinned[5];
-			TRACE_SUB(3);
-			if (nlong > 0)
-				k_bpc_sum_long<<<(nlong + BPC_LWARPS - 1)/BPC_LWARPS, 32*BPC_LWARPS, 0, st>>>(d_lperm, ukeys, ucnt, uoff, nlong, vals_out,
-				  B.post, colbits, ld);
-			if (nruns > nlong)
-				k_bpc_sum_short<<<(nruns - nlong + 127)/128, 128, 0, st>>>(d_lperm, ukeys, ucnt, uoff, nlong, nruns, vals_out, B.post, colbits, ld);
-			CU(cudaGetLastError());
-			TRACE_SUB(4);
-			TRACE_MARK(2);
-			ctx->stats.kernel_launches += 14;
+			M.boff[m - na] = M.btot;
+			M.btot += ctx->h_len[s];
 			}
 		}
-	else
-		{
-	// the accumulator rows of BP_WARPS warps + their cp.async double buffers must fit in shared memory
-	const size_t acc_smem = (((size_t) BP_WARPS*cols_b*sizeof(float) + 15) & ~(size_t) 15) + (size_t) BP_WARPS*BP_NBUF*BP_G*BP_W*sizeof(uint2);
-	if (acc_smem > 220*1024)
-		return mb_fail(ctx, MB200_EOVERFLOW, "alignment with %u columns too wide for the BuildPost kernel", cols_b);
-	// batches of sequences of A sized so that the staging area (one slot per residue of the batch and
-	// member of B) stays below ~2 GB
-	const uint64_t budget_slots = (2048ull << 20)/(BP_W*sizeof(uint2));
-	uint64_t max_slots = 0;
-	std::vector<uint32_t> cuts(1, 0);
+	return MB200_OK;
+	}
+// Carves the copies out of ctx->d_join, followed by `extra` bytes from `rest` on; uploads ids, boff and rb
+static int upload_members(mb200_ctx *ctx, JoinMembers &M, uint32_t c2p_cols, size_t extra, JoinTimer &T, char *&rest)
+	{
+	const size_t na = M.na, nb = M.nb;
+	ENSURE(ctx->d_join, al256((na + nb)*4) + al256((na + 1)*4) + al256(nb*8) + al256(na*c2p_cols*4) + al256(M.btot*4) + extra);
+	char *p = (char *) ctx->d_join.p;
+	M.d_ids = (uint32_t *) p;            p += al256((na + nb)*4);
+	M.d_rb = (uint32_t *) p;             p += al256((na + 1)*4);
+	M.d_boff = (uint64_t *) p;           p += al256(nb*8);
+	M.d_c2p = (int32_t *) p;             p += al256(na*c2p_cols*4);
+	M.d_p2cb = (uint32_t *) p;           p += al256(M.btot*4);
+	rest = p;
+	T.mark(5);
+	CU(cudaMemcpyAsync(M.d_ids, M.ids.data(), (na + nb)*4, cudaMemcpyHostToDevice, ctx->stream));
+	CU(cudaMemcpyAsync(M.d_boff, M.boff.data(), nb*8, cudaMemcpyHostToDevice, ctx->stream));
+	CU(cudaMemcpyAsync(M.d_rb, M.h_rb.data(), (na + 1)*4, cudaMemcpyHostToDevice, ctx->stream));
+	ctx->stats.h2d_bytes += (na + nb)*4 + nb*8;
+	return MB200_OK;
+	}
+// A's members cut into batches of at most `budget` (residue of A, member of B) rows, at least one
+// member each: batch b is members cuts[b] .. cuts[b+1]-1
+struct MemberBatches
+	{
+	std::vector<uint32_t> cuts;
+	uint64_t max_rows = 0;           // rows and residues of the largest batch
+	uint32_t max_res = 0;
+	};
+static MemberBatches member_batches(const std::vector<uint32_t> &h_rb, uint32_t nb, uint64_t budget)
+	{
+	MemberBatches bt;
+	bt.cuts.push_back(0);
+	const uint32_t na = (uint32_t) h_rb.size() - 1;
 	for (uint32_t s = 0; s < na; )
 		{
 		uint32_t e = s + 1;
-		while (e < na && (uint64_t)(h_rb[e + 1] - h_rb[s])*nb <= budget_slots)
+		while (e < na && (uint64_t)(h_rb[e + 1] - h_rb[s])*nb <= budget)
 			++e;
-		max_slots = std::max<uint64_t>(max_slots, (uint64_t)(h_rb[e] - h_rb[s])*nb);
-		cuts.push_back(e);
+		bt.max_rows = std::max<uint64_t>(bt.max_rows, (uint64_t)(h_rb[e] - h_rb[s])*nb);
+		bt.max_res = std::max(bt.max_res, h_rb[e] - h_rb[s]);
+		bt.cuts.push_back(e);
 		s = e;
 		}
-	ENSURE(ctx->d_stage, max_slots*BP_W*sizeof(uint2) + 256);
-	nbatches = cuts.size() - 1;
+	return bt;
+	}
+// BuildPost with the terms bucketed by output cell (k_bpc_*).  Scratch: d_tmp (per residue and row of a batch),
+// d_stage (per term), d_tmp2 (per run).  Reads back through ctx->h_pinned[4] (terms, then runs) and [5] (long runs).
+static int buildpost_by_cell(mb200_ctx *ctx, const BuildPostParams &P, const uint32_t *d_rb, const std::vector<uint32_t> &h_rb,
+  const MemberBatches &bt, uint32_t colbits, uint32_t rowbits, JoinTimer &T)
+	{
+	cudaStream_t st = ctx->stream;
+	if (bt.max_rows >= 0x7ffffff0ull)
+		return mb_fail(ctx, MB200_EOVERFLOW, "BuildPost batch of %llu rows", (unsigned long long) bt.max_rows);
+	// d_tmp: rowof, seqof [residues] | cnt [max_rows+1] | off [max_rows+1] | eptr [max_rows] | 5 x [max_res] | nruns | cub scratch
+	const size_t rowof_b = al256((size_t) h_rb[P.na]*4), rt_b = al256((size_t)(bt.max_rows + 1)*4), res_b = al256((size_t) bt.max_res*4);
+	size_t scan_tb = 0, rsort_tb = 0;
+	cub::DeviceScan::ExclusiveSum(nullptr, scan_tb, (const uint32_t *) nullptr, (uint32_t *) nullptr, (int)(bt.max_rows + 1), st);
+	cub::DeviceRadixSort::SortPairs(nullptr, rsort_tb, (const uint32_t *) nullptr, (uint32_t *) nullptr,
+	  (const uint32_t *) nullptr, (uint32_t *) nullptr, (int) bt.max_res, 0, (int) rowbits, st);
+	const size_t tb1 = al256(std::max(scan_tb, rsort_tb));
+	ENSURE(ctx->d_tmp, 2*rowof_b + 4*rt_b + 5*res_b + 256 + tb1);
+	char *tp = (char *) ctx->d_tmp.p;
+	uint32_t *d_rowof = (uint32_t *) tp;             tp += rowof_b;
+	uint32_t *d_seqof = (uint32_t *) tp;             tp += rowof_b;
+	uint64_t *d_eptr = (uint64_t *) tp;              tp += 2*rt_b;
+	uint32_t *d_cnt = (uint32_t *) tp;               tp += rt_b;
+	uint32_t *d_off = (uint32_t *) tp;               tp += rt_b;
+	uint32_t *d_rk = (uint32_t *) tp;                tp += res_b;      // row of the residue / sorted
+	uint32_t *d_ri = (uint32_t *) tp;                tp += res_b;      // local index
+	uint32_t *d_rk2 = (uint32_t *) tp;               tp += res_b;
+	uint32_t *d_perm = (uint32_t *) tp;              tp += res_b;      // residues in (row, s) order
+	uint32_t *d_base = (uint32_t *) tp;              tp += res_b;
+	uint32_t *d_nruns = (uint32_t *) tp;             tp += 256;
+	void *d_scratch1 = tp;
+	k_bp_rowof<<<dim3((P.cols_a + 255)/256, P.na), 256, 0, st>>>(P, d_rb, d_rowof, d_seqof);
+	CU(cudaGetLastError());
+	const int sms = ctx->prop.multiProcessorCount;
+	for (size_t b = 0; b + 1 < bt.cuts.size(); ++b)
+		{
+		T.tsub = now_s();
+		BpCells C;
+		C.s_lo = bt.cuts[b]; C.s_n = bt.cuts[b + 1] - bt.cuts[b];
+		C.rb = d_rb; C.rowof = d_rowof; C.seqof = d_seqof; C.cnt = d_cnt; C.eptr = d_eptr; C.off = d_off; C.base = d_base;
+		C.colbits = colbits;
+		C.keys = nullptr; C.vals = nullptr;
+		const uint32_t nres = h_rb[bt.cuts[b + 1]] - h_rb[bt.cuts[b]];
+		const uint64_t rt = (uint64_t) nres*P.nb;
+		const uint32_t gblocks = (uint32_t) std::min<uint64_t>((rt + 255)/256, (uint64_t) sms*32);
+		const uint32_t rblocks = (nres + 255)/256;
+		k_bpc_count<<<gblocks, 256, 0, st>>>(P, C);
+		CU(cudaMemsetAsync(d_cnt + rt, 0, 4, st));
+		size_t t0 = tb1;
+		cub::DeviceScan::ExclusiveSum(d_scratch1, t0, (const uint32_t *) d_cnt, d_off, (int)(rt + 1), st);
+		CU(cudaGetLastError());
+		CU(cudaMemcpyAsync(ctx->h_pinned + 4, d_off + rt, 4, cudaMemcpyDeviceToHost, st));
+		// residues ordered by (row, s): the input order is s-major, the sort is stable
+		k_bpc_reskeys<<<rblocks, 256, 0, st>>>(nres, d_rowof + h_rb[bt.cuts[b]], d_rk, d_ri);
+		t0 = tb1;
+		cub::DeviceRadixSort::SortPairs(d_scratch1, t0, (const uint32_t *) d_rk, d_rk2, (const uint32_t *) d_ri, d_perm,
+		  (int) nres, 0, (int) rowbits, st);
+		k_bpc_resterms<<<rblocks, 256, 0, st>>>(nres, P.nb, d_perm, d_off, d_rk);           // d_rk: terms per residue, sorted order
+		t0 = tb1;
+		cub::DeviceScan::ExclusiveSum(d_scratch1, t0, (const uint32_t *) d_rk, d_rk2, (int) nres, st);
+		k_bpc_resbase<<<rblocks, 256, 0, st>>>(nres, d_perm, d_rk2, d_base);
+		CU(cudaGetLastError());
+		CU(cudaStreamSynchronize(st));
+		const uint64_t M = ctx->h_pinned[4];
+		if (M >= 0x7fffffffull)
+			return mb_fail(ctx, MB200_EOVERFLOW, "BuildPost batch of %llu terms", (unsigned long long) M);
+		if (M == 0)
+			continue;
+		// d_stage: keys_in | vals_in | keys_out | vals_out | run offsets | cub scratch
+		const size_t mb = al256((size_t) M*4);
+		size_t sort_tb = 0, rle_tb = 0, scan2_tb = 0;
+		cub::DeviceRadixSort::SortPairs(nullptr, sort_tb, (const uint32_t *) nullptr, (uint32_t *) nullptr,
+		  (const float *) nullptr, (float *) nullptr, (int) M, 0, (int) colbits, st);
+		cub::DeviceRunLengthEncode::Encode(nullptr, rle_tb, (const uint32_t *) nullptr, (uint32_t *) nullptr, (uint32_t *) nullptr,
+		  (uint32_t *) nullptr, (int) M, st);
+		cub::DeviceScan::ExclusiveSum(nullptr, scan2_tb, (const uint32_t *) nullptr, (uint32_t *) nullptr, (int) M, st);
+		const size_t tb = std::max(sort_tb, std::max(rle_tb, scan2_tb));
+		ENSURE(ctx->d_stage, 5*mb + al256(tb) + 256);
+		char *sp = (char *) ctx->d_stage.p;
+		uint32_t *keys_in = (uint32_t *) sp;              float *vals_in = (float *)(sp + mb);
+		uint32_t *keys_out = (uint32_t *)(sp + 2*mb);     float *vals_out = (float *)(sp + 3*mb);
+		uint32_t *uoff = (uint32_t *)(sp + 4*mb);
+		void *scratch2 = sp + 5*mb;
+		C.keys = keys_in; C.vals = vals_in;
+		T.sub(0);
+		k_bpc_emit<<<(uint32_t) std::min<uint64_t>((rt*8 + 255)/256, (uint64_t) sms*32), 256, 0, st>>>(P, C);
+		CU(cudaGetLastError());
+		T.sub(1);
+		T.mark(1);
+		// stable sort on the column bits only: (row, s, t) order survives inside every column
+		size_t t1 = sort_tb;
+		cub::DeviceRadixSort::SortPairs(scratch2, t1, (const uint32_t *) keys_in, keys_out, (const float *) vals_in, vals_out,
+		  (int) M, 0, (int) colbits, st);
+		T.sub(2);
+		// runs of equal cells: unique keys and lengths reuse the input buffers
+		uint32_t *ukeys = keys_in, *ucnt = (uint32_t *) vals_in;
+		size_t t2 = rle_tb;
+		cub::DeviceRunLengthEncode::Encode(scratch2, t2, (const uint32_t *) keys_out, ukeys, ucnt, d_nruns, (int) M, st);
+		CU(cudaGetLastError());
+		CU(cudaMemcpyAsync(ctx->h_pinned + 4, d_nruns, 4, cudaMemcpyDeviceToHost, st));
+		CU(cudaStreamSynchronize(st));
+		const uint32_t nruns = ctx->h_pinned[4];
+		size_t t3 = scan2_tb;
+		cub::DeviceScan::ExclusiveSum(scratch2, t3, (const uint32_t *) ucnt, uoff, (int) nruns, st);
+		// runs by descending length (d_tmp2: counts out | index in | index out | cub scratch)
+		size_t lsort_tb = 0;
+		cub::DeviceRadixSort::SortPairsDescending(nullptr, lsort_tb, (const uint32_t *) nullptr, (uint32_t *) nullptr,
+		  (const uint32_t *) nullptr, (uint32_t *) nullptr, (int) nruns, 0, 32, st);
+		const size_t nrb = al256((size_t) nruns*4);
+		ENSURE(ctx->d_tmp2, 3*nrb + al256(lsort_tb));
+		uint32_t *d_lc = (uint32_t *) ctx->d_tmp2.p;
+		uint32_t *d_li = (uint32_t *)((char *) ctx->d_tmp2.p + nrb);
+		uint32_t *d_lperm = (uint32_t *)((char *) ctx->d_tmp2.p + 2*nrb);
+		void *d_lscratch = (char *) ctx->d_tmp2.p + 3*nrb;
+		k_iota<<<(nruns + 255)/256, 256, 0, st>>>(nruns, d_li);
+		cub::DeviceRadixSort::SortPairsDescending(d_lscratch, lsort_tb, (const uint32_t *) ucnt, d_lc, (const uint32_t *) d_li, d_lperm,
+		  (int) nruns, 0, 32, st);
+		k_count_ge<<<1, 1, 0, st>>>(d_lc, nruns, BPC_LONG, d_nruns + 1);
+		CU(cudaMemcpyAsync(ctx->h_pinned + 5, d_nruns + 1, 4, cudaMemcpyDeviceToHost, st));
+		CU(cudaStreamSynchronize(st));
+		const uint32_t nlong = ctx->h_pinned[5];
+		T.sub(3);
+		if (nlong > 0)
+			k_bpc_sum_long<<<(nlong + BPC_LWARPS - 1)/BPC_LWARPS, 32*BPC_LWARPS, 0, st>>>(d_lperm, ukeys, ucnt, uoff, nlong, vals_out,
+			  P.post, colbits, P.ld);
+		if (nruns > nlong)
+			k_bpc_sum_short<<<(nruns - nlong + 127)/128, 128, 0, st>>>(d_lperm, ukeys, ucnt, uoff, nlong, nruns, vals_out, P.post, colbits, P.ld);
+		CU(cudaGetLastError());
+		T.sub(4);
+		T.mark(2);
+		ctx->stats.kernel_launches += 14;
+		}
+	return MB200_OK;
+	}
+// BuildPost as an ordered walk over the rows (k_bp_gather / k_bp_apply).  Scratch: d_stage, d_tmp2.  No read-backs.
+static int buildpost_by_row(mb200_ctx *ctx, const BuildPostParams &P, const uint32_t *d_rb, const std::vector<uint32_t> &h_rb,
+  const MemberBatches &bt, JoinTimer &T)
+	{
+	cudaStream_t st = ctx->stream;
+	const uint32_t cols_a = P.cols_a;
+	// the accumulator rows of BP_WARPS warps + their cp.async double buffers must fit in shared memory
+	const size_t acc_smem = (((size_t) BP_WARPS*P.cols_b*sizeof(float) + 15) & ~(size_t) 15) + (size_t) BP_WARPS*BP_NBUF*BP_G*BP_W*sizeof(uint2);
+	if (acc_smem > 220*1024)
+		return mb_fail(ctx, MB200_EOVERFLOW, "alignment with %u columns too wide for the BuildPost kernel", P.cols_b);
+	ENSURE(ctx->d_stage, bt.max_rows*BP_W*sizeof(uint2) + 256);
 	BpStage G;
 	G.slots = (uint2 *) ctx->d_stage.p;
 	G.rb = d_rb;
@@ -1375,68 +1436,84 @@ static int join_core(mb200_ctx *ctx, uint32_t na, uint32_t nb, const uint32_t *d
 	CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_bp_apply, 32*BP_WARPS, acc_smem));
 	const uint32_t ablocks = std::max<uint32_t>(1, std::min<uint32_t>((cols_a + BP_WARPS - 1)/BP_WARPS,
 	  (uint32_t) std::max(occ, 1)*ctx->prop.multiProcessorCount));
-	for (size_t b = 0; b + 1 < cuts.size(); ++b)
+	for (size_t b = 0; b + 1 < bt.cuts.size(); ++b)
 		{
-		G.s_lo = cuts[b];
-		G.s_n = cuts[b + 1] - cuts[b];
-		const uint64_t total = (uint64_t)(h_rb[cuts[b + 1]] - h_rb[cuts[b]])*nb;
+		G.s_lo = bt.cuts[b];
+		G.s_n = bt.cuts[b + 1] - bt.cuts[b];
+		const uint64_t total = (uint64_t)(h_rb[bt.cuts[b + 1]] - h_rb[bt.cuts[b]])*P.nb;
 		const uint32_t gblocks = (uint32_t) std::min<uint64_t>((total + 255)/256, (uint64_t) ctx->prop.multiProcessorCount*32);
 		k_bp_gather<<<gblocks, 256, 0, st>>>(P, G);
-		TRACE_MARK(1);
+		T.mark(1);
 		CU(cudaMemsetAsync(d_cursor, 0, 4, st));
 		k_bp_apply<<<ablocks, 32*BP_WARPS, acc_smem, st>>>(P, G, S);
-		TRACE_MARK(2);
+		T.mark(2);
 		ctx->stats.kernel_launches += 2;
 		}
 	ctx->stats.kernel_launches += 2;
 	CU(cudaGetLastError());
-		}
-	AlnProblem pr;
-	pr.LX = cols_a; pr.LY = cols_b; pr.ld = ld; pr.dense = B.post; pr.tb = B.tb; pr.edge = B.edge;
-	pr.done = (uint32_t *)((char *) B.edge + chan_bytes - 256);
-	if (npass > 1)
-		CU(cudaMemsetAsync(B.edge, 0, chan_bytes, st));
-	pr.path = B.path; pr.score = B.score; pr.plen = B.plen;
-	CU(cudaMemcpyAsync(B.prob, &pr, sizeof pr, cudaMemcpyHostToDevice, st));
-	if (tb_smem)
-		{
-		CU(cudaFuncSetAttribute(k_aln_wave<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) std::max<size_t>(tbw, 16)));
-		k_aln_wave<true><<<1, 32*nwarps, tbw, st>>>(B.prob);
-		}
-	else
-		k_aln_wave<false><<<dim3(1, npass), 32*nwarps, 0, st>>>(B.prob);
-	CU(cudaGetLastError());
-	ctx->stats.kernel_launches++;
-	const double g1 = g_t[1], g2 = g_t[2], g3 = g_t[3];
-	TRACE_MARK(3);
-	if (g_trace_level >= 2 && na + nb >= 64)
-		fprintf(stderr, "[mb200 join] %u x %u seqs, %u x %u cols, %zu batch(es): DP %.2f ms (BuildPost totals so far: gather %.1f ms apply %.1f ms)\n",
-		  na, nb, cols_a, cols_b, nbatches, 1e3*(g_t[3] - g3), 1e3*g1, 1e3*g2);
 	return MB200_OK;
 	}
 
-static size_t join_scratch_bytes(uint32_t cols_a, uint32_t cols_b)
+// BuildPost + decoding DP of a join whose members and maps are on the device.  Fills pr (the matrix,
+// path, score and plen stay on the device) and does NOT synchronise.
+static int join_core(mb200_ctx *ctx, const JoinMembers &M, uint32_t cols_a, uint32_t cols_b, char *scratch, size_t scratch_bytes,
+  AlnProblem &pr, JoinTimer &T)
 	{
-	const uint32_t ld = (cols_b + AW_C - 1)/AW_C*AW_C;
-	const uint32_t nstrips = (cols_b + AW_W - 1)/AW_W;
-	return al256(aw_dense_bytes(cols_a, ld)) + al256((size_t) cols_a*nstrips*32) + al256((size_t)(nstrips/AW_MAXW + 1)*((size_t) cols_a + 1)*8 + 256)
-	  + al256((size_t) cols_a + cols_b + 16) + 4*256;
-	}
+	cudaStream_t st = ctx->stream;
+	const uint32_t na = M.na, nb = M.nb;
+	const AlnLayout L = aln_layout(cols_a, cols_b, true);
+	if (L.bytes() > scratch_bytes)
+		return mb_fail(ctx, MB200_EINVAL, "join scratch too small");
+	char *tb = scratch + al256(L.dense_bytes), *chan = tb + L.tb_carve(), *path = chan + L.chan_bytes;
+	char *tail = path + al256(L.path_bytes);                       // score | plen | the AlnProblem
+	aln_place(L, scratch, tb, chan, path, pr);
+	pr.score = (float *) tail; pr.plen = (uint32_t *)(tail + 256);
+	AlnProblem *d_prob = (AlnProblem *)(tail + 512);
+	CU(cudaMemsetAsync(scratch, 0, L.dense_bytes, st));
 
-static int need_store_for_joins(mb200_ctx *ctx, const char *who)
-	{
-	if (!ctx->store_valid || !ctx->store_allpairs)
-		return mb_fail(ctx, MB200_EINVAL, "%s: the store must hold all N(N-1)/2 pairs", who);
-	int rc = mb_store_build_transposed(ctx);
+	BuildPostParams P;
+	P.n = ctx->nseq; P.na = na; P.nb = nb; P.cols_a = cols_a; P.cols_b = cols_b; P.ld = L.ld;
+	P.ids_a = M.d_ids; P.ids_b = M.d_ids + na; P.col2pos_a = M.d_c2p; P.p2c_b = M.d_p2cb; P.p2c_b_off = M.d_boff;
+	P.rowbase = (const uint64_t *) ctx->d_rowbase.p; P.rowoff = (const uint32_t *) ctx->d_rowoff.p;
+	P.entries = (const mb200_entry *) ctx->d_entries.p;
+	P.trbase = (const uint64_t *) ctx->d_tr_rowbase.p; P.troff = (const uint32_t *) ctx->d_tr_rowoff.p;
+	P.trentries = (const mb200_entry *) ctx->d_tr_entries.p;
+	P.entbase = (const uint64_t *) ctx->d_entbase.p;
+	P.post = (float *) pr.dense;
+	// large joins: bucket the contributions by cell (see k_bpc_*); small ones: ordered row walk (k_bp_apply)
+	const char *ev_sort = getenv("MB200_BP_SORT_MIN");             // tuning hook: (residues of A) x |B| from which to sort
+	const long long sort_min = ev_sort ? atoll(ev_sort) : 1000000ll;
+	uint32_t colbits = 1, rowbits = 1;
+	while ((1u << colbits) < cols_b)
+		++colbits;
+	while ((1u << rowbits) < cols_a)
+		++rowbits;
+	const bool by_cell = (uint64_t) M.h_rb[na]*nb >= (uint64_t) sort_min && colbits + rowbits <= 32 && na <= 65535;
+	// batches of A's members: by cell at most ~16M (residue, t) rows; by row, the staging area (one slot
+	// per residue of the batch and member of B) stays below ~2 GB
+	const MemberBatches bt = member_batches(M.h_rb, nb, by_cell ? 16ull << 20 : (2048ull << 20)/(BP_W*sizeof(uint2)));
+	const int rc = by_cell ? buildpost_by_cell(ctx, P, M.d_rb, M.h_rb, bt, colbits, rowbits, T)
+	  : buildpost_by_row(ctx, P, M.d_rb, M.h_rb, bt, T);
 	if (rc != MB200_OK)
 		return rc;
-	if (ctx->tr_values_stale)
+
+	if (L.npass > 1)
+		CU(cudaMemsetAsync(chan, 0, L.chan_bytes, st));
+	CU(cudaMemcpyAsync(d_prob, &pr, sizeof pr, cudaMemcpyHostToDevice, st));
+	if (L.tb_smem)
 		{
-		rc = mb_store_refresh_transposed(ctx);
-		if (rc != MB200_OK)
-			return rc;
-		ctx->tr_values_stale = false;
+		CU(cudaFuncSetAttribute(k_aln_wave<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) std::max<size_t>(L.tb_bytes, 16)));
+		k_aln_wave<true><<<1, 32*L.nwarps, L.tb_bytes, st>>>(d_prob);
 		}
+	else
+		k_aln_wave<false><<<dim3(1, L.npass), 32*L.nwarps, 0, st>>>(d_prob);
+	CU(cudaGetLastError());
+	ctx->stats.kernel_launches++;
+	const double g1 = g_t[1], g2 = g_t[2], g3 = g_t[3];
+	T.mark(3);
+	if (g_trace_level >= 2 && na + nb >= 64)
+		fprintf(stderr, "[mb200 join] %u x %u seqs, %u x %u cols, %zu batch(es): DP %.2f ms (BuildPost totals so far: gather %.1f ms apply %.1f ms)\n",
+		  na, nb, cols_a, cols_b, bt.cuts.size() - 1, 1e3*(g_t[3] - g3), 1e3*g1, 1e3*g2);
 	return MB200_OK;
 	}
 
@@ -1455,6 +1532,7 @@ int mb200_align_pairs(mb200_ctx *ctx, uint32_t n, const uint32_t *store_pairs, c
 	const uint32_t np = (uint32_t) ctx->h_px.size();
 	std::vector<AlnProblem> probs(n);
 	std::vector<DensifyJob> jobs(n);
+	std::vector<AlnLayout> lay(n);
 	uint64_t dense_total = 0, tb_total = 0, edge_total = 0;
 	const uint64_t path_total = path_off[n];
 	uint32_t lxmax = 0, maxstrips = 1;
@@ -1466,13 +1544,14 @@ int mb200_align_pairs(mb200_ctx *ctx, uint32_t n, const uint32_t *store_pairs, c
 		const uint32_t LX = ctx->h_len[ctx->h_px[sp]], LY = ctx->h_len[ctx->h_py[sp]];
 		if (path_off[k + 1] < path_off[k] + LX + LY + 1)
 			return mb_fail(ctx, MB200_EINVAL, "path_off[%u..%u] leaves less than LX+LY+1 bytes", k, k + 1);
-		const uint32_t ld = (LY + AW_C - 1)/AW_C*AW_C;
-		const uint32_t nstrips = (LY + AW_W - 1)/AW_W;
-		dense_total += al256(aw_dense_bytes(LX, ld));
-		tb_total += al256((uint64_t) LX*nstrips*32);
-		edge_total += al256((uint64_t)(nstrips/AW_MAXW + 1)*((uint64_t) LX + 1)*8 + 256);
+		// the batch launch below keeps every traceback in global memory; with nwarps = min(AW_MAXW, nstrips)
+		// each problem's npass is the one k_aln_wave derives from the launch's min(AW_MAXW, maxstrips) warps
+		lay[k] = aln_layout(LX, LY, false);
+		dense_total += al256(lay[k].dense_bytes);
+		tb_total += lay[k].tb_carve();
+		edge_total += lay[k].chan_bytes;
 		lxmax = std::max(lxmax, LX);
-		maxstrips = std::max(maxstrips, nstrips);
+		maxstrips = std::max(maxstrips, lay[k].nstrips);
 		}
 	const size_t need = dense_total + tb_total + edge_total + al256(path_total + 16) + al256(n*sizeof(float))
 	  + al256(n*sizeof(AlnProblem)) + al256(n*sizeof(DensifyJob));
@@ -1489,26 +1568,19 @@ int mb200_align_pairs(mb200_ctx *ctx, uint32_t n, const uint32_t *store_pairs, c
 	for (uint32_t k = 0; k < n; ++k)
 		{
 		const uint32_t sp = store_pairs[k];
-		const uint32_t LX = ctx->h_len[ctx->h_px[sp]], LY = ctx->h_len[ctx->h_py[sp]];
-		const uint32_t ld = (LY + AW_C - 1)/AW_C*AW_C;
-		const uint32_t nstrips = (LY + AW_W - 1)/AW_W;
+		const AlnLayout &L = lay[k];
 		AlnProblem &q = probs[k];
-		q.LX = LX; q.LY = LY; q.ld = ld;
-		q.dense = (const float *)(d_dense + od) + ld;
-		q.tb = (uint8_t *)(d_tb + ot);
-		q.edge = (uint2 *)(d_edge + oe);
-		q.done = (uint32_t *)(d_edge + oe + al256((uint64_t)(nstrips/AW_MAXW + 1)*((uint64_t) LX + 1)*8 + 256) - 256);
-		q.path = d_paths + path_off[k];
+		aln_place(L, d_dense + od, d_tb + ot, d_edge + oe, d_paths + path_off[k], q);
 		q.score = d_scores + k;
 		q.plen = nullptr;
 		DensifyJob &j = jobs[k];
 		j.rowoff = (const uint32_t *) ctx->d_rowoff.p + ctx->h_rowbase[sp];
 		j.entries = (const mb200_entry *) ctx->d_entries.p + ctx->h_entbase[sp];
-		j.dense = (float *)(d_dense + od) + ld;
-		j.LX = LX; j.ld = ld;
-		od += al256(aw_dense_bytes(LX, ld));
-		ot += al256((uint64_t) LX*nstrips*32);
-		oe += al256((uint64_t)(nstrips/AW_MAXW + 1)*((uint64_t) LX + 1)*8 + 256);
+		j.dense = (float *) q.dense;
+		j.LX = L.LX; j.ld = L.ld;
+		od += al256(L.dense_bytes);
+		ot += L.tb_carve();
+		oe += L.chan_bytes;
 		}
 	CU(cudaMemsetAsync(d_dense, 0, dense_total, st));
 	CU(cudaMemcpyAsync(d_probs, probs.data(), n*sizeof(AlnProblem), cudaMemcpyHostToDevice, st));
@@ -1538,80 +1610,45 @@ int mb200_align_groups(mb200_ctx *ctx, uint32_t na, const uint32_t *ids_a, const
 		return mb_fail(ctx, MB200_EINVAL, "mb200_align_groups: bad argument");
 	cudaSetDevice(ctx->device);
 	cudaStream_t st = ctx->stream;
-	trace_init();
-	int rc = need_store_for_joins(ctx, "mb200_align_groups");
+	JoinMembers M;
+	int rc = join_members(ctx, "mb200_align_groups", na, ids_a, nb, ids_b, M);
 	if (rc != MB200_OK)
 		return rc;
-	double tmark = now_s();
-	++g_calls;
+	JoinTimer T(st);
 	// host-side index maps (tiny): col->pos for A, concatenated pos->col for B; validated here
-	std::vector<uint8_t> member(ctx->nseq, 0);
 	std::vector<int32_t> c2p((size_t) na*cols_a, -1);
-	uint64_t off = 0;
 	for (uint32_t s = 0; s < na; ++s)
-		{
-		if (ids_a[s] >= ctx->nseq || member[ids_a[s]])
-			return mb_fail(ctx, MB200_EINVAL, "group A sequence id out of range or repeated");
-		member[ids_a[s]] = 1;
-		const uint32_t L = ctx->h_len[ids_a[s]];
-		for (uint32_t i = 0; i < L; ++i)
+		for (uint32_t i = 0; i < M.h_rb[s + 1] - M.h_rb[s]; ++i)
 			{
-			const uint32_t c = pos2col_a[off + i];
+			const uint32_t c = pos2col_a[M.h_rb[s] + i];
 			if (c >= cols_a)
-				return mb_fail(ctx, MB200_EINVAL, "group A pos2col out of range");
+				return mb_fail(ctx, MB200_EINVAL, "mb200_align_groups: group A pos2col out of range");
 			c2p[(size_t) s*cols_a + c] = (int32_t) i;
 			}
-		off += L;
-		}
-	std::vector<uint32_t> h_rb(na + 1, 0);
-	for (uint32_t s = 0; s < na; ++s)
-		h_rb[s + 1] = h_rb[s] + ctx->h_len[ids_a[s]];
-	std::vector<uint64_t> boff(nb);
-	uint64_t btot = 0;
-	for (uint32_t t = 0; t < nb; ++t)
-		{
-		if (ids_b[t] >= ctx->nseq || member[ids_b[t]])
-			return mb_fail(ctx, MB200_EINVAL, "group B sequence id out of range, repeated, or also in group A "
-			  "(the reference asserts SMI_1 != SMI_2, buildpostflat.cpp:49)");
-		member[ids_b[t]] = 1;
-		boff[t] = btot;
-		const uint32_t L = ctx->h_len[ids_b[t]];
-		for (uint32_t i = 0; i < L; ++i)
-			if (pos2col_b[btot + i] >= cols_b)
-				return mb_fail(ctx, MB200_EINVAL, "group B pos2col out of range");
-		btot += L;
-		}
-	const size_t maps = al256(c2p.size()*4) + al256(btot*4) + al256(nb*8) + al256(na*4) + al256(nb*4) + al256((na + 1)*4);
-	const size_t jsz = join_scratch_bytes(cols_a, cols_b);
-	ENSURE(ctx->d_join, maps + jsz);
-	char *base = (char *) ctx->d_join.p;
-	int32_t *d_c2p = (int32_t *) base;               base += al256(c2p.size()*4);
-	uint32_t *d_p2cb = (uint32_t *) base;            base += al256(btot*4);
-	uint64_t *d_boff = (uint64_t *) base;            base += al256(nb*8);
-	uint32_t *d_ida = (uint32_t *) base;             base += al256(na*4);
-	uint32_t *d_idb = (uint32_t *) base;             base += al256(nb*4);
-	uint32_t *d_rb = (uint32_t *) base;              base += al256((na + 1)*4);
-	TRACE_MARK(5);
-	CU(cudaMemcpyAsync(d_rb, h_rb.data(), (na + 1)*4, cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(d_c2p, c2p.data(), c2p.size()*4, cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(d_p2cb, pos2col_b, btot*4, cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(d_boff, boff.data(), nb*8, cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(d_ida, ids_a, na*4, cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(d_idb, ids_b, nb*4, cudaMemcpyHostToDevice, st));
-	ctx->stats.h2d_bytes += c2p.size()*4 + btot*4 + nb*8 + (na + nb)*4;
-	TRACE_MARK(0);
-	JoinBufs B;
-	rc = join_core(ctx, na, nb, d_ida, d_idb, d_c2p, d_p2cb, d_boff, d_rb, h_rb, cols_a, cols_b, base, jsz, B, tmark);
+	for (uint64_t i = 0; i < M.btot; ++i)
+		if (pos2col_b[i] >= cols_b)
+			return mb_fail(ctx, MB200_EINVAL, "mb200_align_groups: group B pos2col out of range");
+	const size_t jsz = aln_layout(cols_a, cols_b, true).bytes();
+	char *scratch = nullptr;
+	rc = upload_members(ctx, M, cols_a, jsz, T, scratch);
 	if (rc != MB200_OK)
 		return rc;
-	CU(cudaMemcpyAsync(path_out, B.path, cols_a + cols_b + 1, cudaMemcpyDeviceToHost, st));
+	CU(cudaMemcpyAsync(M.d_c2p, c2p.data(), c2p.size()*4, cudaMemcpyHostToDevice, st));
+	CU(cudaMemcpyAsync(M.d_p2cb, pos2col_b, M.btot*4, cudaMemcpyHostToDevice, st));
+	ctx->stats.h2d_bytes += c2p.size()*4 + M.btot*4;
+	T.mark(0);
+	AlnProblem pr;
+	rc = join_core(ctx, M, cols_a, cols_b, scratch, jsz, pr, T);
+	if (rc != MB200_OK)
+		return rc;
+	CU(cudaMemcpyAsync(path_out, pr.path, cols_a + cols_b + 1, cudaMemcpyDeviceToHost, st));
 	if (score_out)
-		CU(cudaMemcpyAsync(score_out, B.score, sizeof(float), cudaMemcpyDeviceToHost, st));
+		CU(cudaMemcpyAsync(score_out, pr.score, sizeof(float), cudaMemcpyDeviceToHost, st));
 	if (post_out)
-		CU(cudaMemcpy2DAsync(post_out, (size_t) cols_b*sizeof(float), B.post, (size_t) B.ld*sizeof(float),
+		CU(cudaMemcpy2DAsync(post_out, (size_t) cols_b*sizeof(float), pr.dense, (size_t) pr.ld*sizeof(float),
 		  (size_t) cols_b*sizeof(float), cols_a, cudaMemcpyDeviceToHost, st));
 	CU(cudaStreamSynchronize(st));
-	TRACE_MARK(5);
+	T.mark(5);
 	ctx->stats.d2h_bytes += cols_a + cols_b + 1 + 4 + (post_out ? (size_t) cols_a*cols_b*4 : 0);
 	return MB200_OK;
 	}
@@ -1635,6 +1672,7 @@ int mb200_msa_reset(mb200_ctx *ctx)
 	return MB200_OK;
 	}
 
+// ctx->h_pinned: words 0-1 projected column counts, 2 path length, 3 score (4-5: buildpost_by_cell)
 int mb200_msa_join(mb200_ctx *ctx, uint32_t na, const uint32_t *ids_a, uint32_t nb, const uint32_t *ids_b,
   uint32_t *cols_out, float *score_out, char *path_out, uint32_t path_cap)
 	{
@@ -1644,73 +1682,36 @@ int mb200_msa_join(mb200_ctx *ctx, uint32_t na, const uint32_t *ids_a, uint32_t 
 		return mb_fail(ctx, MB200_EINVAL, "mb200_msa_join: call mb200_msa_reset first");
 	cudaSetDevice(ctx->device);
 	cudaStream_t st = ctx->stream;
-	trace_init();
-	int rc = need_store_for_joins(ctx, "mb200_msa_join");
+	// members: every id once; all of A in one MSA (same column count), all of B in one MSA
+	JoinMembers M;
+	int rc = join_members(ctx, "mb200_msa_join", na, ids_a, nb, ids_b, M);
 	if (rc != MB200_OK)
 		return rc;
-	double tmark = now_s();
-	++g_calls;
-	// members: every id once; all of A in one MSA (same column count), all of B in one MSA
-	std::vector<uint8_t> member(ctx->nseq, 0);
-	std::vector<uint32_t> ids(na + nb);
-	std::vector<uint64_t> boff(nb);
-	std::vector<uint32_t> h_rb(na + 1, 0);
-	uint32_t lmax = 0;
-	uint64_t btot = 0;
-	for (uint32_t m = 0; m < na + nb; ++m)
-		{
-		const uint32_t s = m < na ? ids_a[m] : ids_b[m - na];
-		if (s >= ctx->nseq || member[s])
-			return mb_fail(ctx, MB200_EINVAL, "mb200_msa_join: sequence id %u out of range or listed twice", s);
-		member[s] = 1;
-		ids[m] = s;
-		lmax = std::max(lmax, ctx->h_len[s]);
-		if (m < na)
-			h_rb[m + 1] = h_rb[m] + ctx->h_len[s];
-		if (m >= na)
-			{
-			boff[m - na] = btot;
-			btot += ctx->h_len[s];
-			}
-		}
+	JoinTimer T(st);
 	const uint32_t old_a = ctx->h_msa_cols[ids_a[0]], old_b = ctx->h_msa_cols[ids_b[0]];
-	for (uint32_t m = 0; m < na; ++m)
-		if (ctx->h_msa_cols[ids_a[m]] != old_a)
-			return mb_fail(ctx, MB200_EINVAL, "mb200_msa_join: group A members are not in one MSA");
-	for (uint32_t m = 0; m < nb; ++m)
-		if (ctx->h_msa_cols[ids_b[m]] != old_b)
-			return mb_fail(ctx, MB200_EINVAL, "mb200_msa_join: group B members are not in one MSA");
+	for (uint32_t m = 0; m < na + nb; ++m)
+		if (ctx->h_msa_cols[M.ids[m]] != (m < na ? old_a : old_b))
+			return mb_fail(ctx, MB200_EINVAL, "mb200_msa_join: group %c members are not in one MSA", m < na ? 'A' : 'B');
 	const uint32_t cap = std::max(old_a, old_b);
-	// fixed part of the scratch: ids, boff, mark/remap [2][cap], map [2][cap], dims
-	const size_t fixed = al256((na + nb)*4) + al256(nb*8) + al256(2*(size_t) cap*4) + al256(2*(size_t) cap*4) + 256
-	  + al256((na + 1)*4);
-	// upper bounds for the projected sizes are the old sizes
-	const size_t mapsz = al256((size_t) na*old_a*4) + al256(btot*4);
-	const size_t jsz = join_scratch_bytes(old_a, old_b);
-	ENSURE(ctx->d_join, fixed + mapsz + jsz);
-	char *base = (char *) ctx->d_join.p;
-	uint32_t *d_ids = (uint32_t *) base;             base += al256((na + nb)*4);
-	uint64_t *d_boff = (uint64_t *) base;            base += al256(nb*8);
-	uint32_t *d_mark = (uint32_t *) base;            base += al256(2*(size_t) cap*4);
-	uint32_t *d_map = (uint32_t *) base;             base += al256(2*(size_t) cap*4);
-	uint32_t *d_dims = (uint32_t *) base;            base += 256;
-	uint32_t *d_rb = (uint32_t *) base;              base += al256((na + 1)*4);
-	int32_t *d_c2p = (int32_t *) base;               base += al256((size_t) na*old_a*4);
-	uint32_t *d_p2cb = (uint32_t *) base;            base += al256(btot*4);
-	TRACE_MARK(5);
-	CU(cudaMemcpyAsync(d_ids, ids.data(), (na + nb)*4, cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(d_boff, boff.data(), nb*8, cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(d_rb, h_rb.data(), (na + 1)*4, cudaMemcpyHostToDevice, st));
+	// after the members: mark/remap [2][cap], map [2][cap], dims, join scratch.  c2p and the join scratch are sized
+	// for the old column counts: the projected ones are no larger, and no size grows as they shrink
+	const size_t jsz = aln_layout(old_a, old_b, true).bytes();
+	char *p = nullptr;
+	rc = upload_members(ctx, M, old_a, 2*al256(2*(size_t) cap*4) + 256 + jsz, T, p);
+	if (rc != MB200_OK)
+		return rc;
+	uint32_t *d_mark = (uint32_t *) p;               p += al256(2*(size_t) cap*4);
+	uint32_t *d_map = (uint32_t *) p;                p += al256(2*(size_t) cap*4);
+	uint32_t *d_dims = (uint32_t *) p;               p += 256;
 	CU(cudaMemsetAsync(d_mark, 0, 2*(size_t) cap*4, st));
-	ctx->stats.h2d_bytes += (na + nb)*4 + nb*8;
 	MsaJob J;
 	memset(&J, 0, sizeof J);
-	J.na = na; J.nb = nb; J.ids = d_ids;
+	J.na = na; J.nb = nb; J.ids = M.d_ids;
 	J.seqoff = (const uint64_t *) ctx->d_seqoff.p; J.seqlen = (const uint32_t *) ctx->d_seqlen.p;
 	J.p2c = (uint32_t *) ctx->d_p2c.p;
 	J.mark = d_mark; J.cap = cap; J.old_cols_a = old_a; J.old_cols_b = old_b; J.dims = d_dims;
 	J.map = d_map;
-	const dim3 mgrid((lmax + 255)/256, na + nb);
+	const dim3 mgrid((M.lmax + 255)/256, na + nb);
 	k_msa_mark<<<mgrid, 256, 0, st>>>(J);
 	k_msa_remap<<<2, 1024, 0, st>>>(J);
 	CU(cudaGetLastError());
@@ -1719,34 +1720,34 @@ int mb200_msa_join(mb200_ctx *ctx, uint32_t na, const uint32_t *ids_a, uint32_t 
 	const uint32_t cols_a = ctx->h_pinned[0], cols_b = ctx->h_pinned[1];
 	if (cols_a == 0 || cols_b == 0 || cols_a > old_a || cols_b > old_b)
 		return mb_fail(ctx, MB200_EINVAL, "mb200_msa_join: projection gave %u x %u columns", cols_a, cols_b);
-	J.c2p_a = d_c2p; J.cols_a = cols_a; J.p2c_b = d_p2cb; J.boff = d_boff;
-	CU(cudaMemsetAsync(d_c2p, 0xff, (size_t) na*cols_a*4, st));
+	J.c2p_a = M.d_c2p; J.cols_a = cols_a; J.p2c_b = M.d_p2cb; J.boff = M.d_boff;
+	CU(cudaMemsetAsync(M.d_c2p, 0xff, (size_t) na*cols_a*4, st));
 	k_msa_maps<<<mgrid, 256, 0, st>>>(J);
 	CU(cudaGetLastError());
 	ctx->stats.kernel_launches += 3;
-	TRACE_MARK(0);
-	JoinBufs B;
-	rc = join_core(ctx, na, nb, d_ids, d_ids + na, d_c2p, d_p2cb, d_boff, d_rb, h_rb, cols_a, cols_b, base, jsz, B, tmark);
+	T.mark(0);
+	AlnProblem pr;
+	rc = join_core(ctx, M, cols_a, cols_b, p, jsz, pr, T);
 	if (rc != MB200_OK)
 		return rc;
-	J.path = B.path; J.plen = B.plen;
+	J.path = pr.path; J.plen = pr.plen;
 	k_msa_pathmap<<<1, 1024, 0, st>>>(J);
 	k_msa_update<<<mgrid, 256, 0, st>>>(J);
 	CU(cudaGetLastError());
 	ctx->stats.kernel_launches += 2;
-	CU(cudaMemcpyAsync(ctx->h_pinned + 2, B.plen, 4, cudaMemcpyDeviceToHost, st));
-	CU(cudaMemcpyAsync(ctx->h_pinned + 3, B.score, 4, cudaMemcpyDeviceToHost, st));
+	CU(cudaMemcpyAsync(ctx->h_pinned + 2, pr.plen, 4, cudaMemcpyDeviceToHost, st));
+	CU(cudaMemcpyAsync(ctx->h_pinned + 3, pr.score, 4, cudaMemcpyDeviceToHost, st));
 	if (path_out)
 		{
 		if (path_cap < cols_a + cols_b + 1)
 			return mb_fail(ctx, MB200_EINVAL, "mb200_msa_join: path buffer of %u bytes, need %u", path_cap, cols_a + cols_b + 1);
-		CU(cudaMemcpyAsync(path_out, B.path, cols_a + cols_b + 1, cudaMemcpyDeviceToHost, st));
+		CU(cudaMemcpyAsync(path_out, pr.path, cols_a + cols_b + 1, cudaMemcpyDeviceToHost, st));
 		}
 	CU(cudaStreamSynchronize(st));
-	TRACE_MARK(4);
+	T.mark(4);
 	const uint32_t newcols = ctx->h_pinned[2];
 	for (uint32_t m = 0; m < na + nb; ++m)
-		ctx->h_msa_cols[ids[m]] = newcols;
+		ctx->h_msa_cols[M.ids[m]] = newcols;
 	if (cols_out)
 		*cols_out = newcols;
 	if (score_out)

@@ -21,10 +21,6 @@ int mb_fail(mb200_ctx *ctx, int code, const char *fmt, ...)
 	return code;
 	}
 
-#define CU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) \
-	return mb_fail(ctx, e_ == cudaErrorMemoryAllocation ? MB200_ENOMEM : MB200_ECUDA, \
-	  "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
-
 int DevBuf::ensure(size_t need)
 	{
 	if (need <= cap)
@@ -65,9 +61,6 @@ void mb_release_post_scratch(mb200_ctx *ctx)
 	for (DevBuf &b : ctx->d_post_scratch)
 		b.release();
 	}
-
-#define ENSURE(buf, bytes) do { if ((buf).ensure(bytes) != 0) \
-	return mb_fail(ctx, MB200_ENOMEM, "device allocation of %zu bytes failed (%s)", (size_t)(bytes), #buf); } while (0)
 
 extern "C" {
 

@@ -97,6 +97,13 @@ struct mb200_ctx
 	};
 
 int mb_fail(mb200_ctx *ctx, int code, const char *fmt, ...);
+// In a host function with a local `ctx` that returns an mb200 error code: fail on a CUDA error / a
+// device allocation that cannot grow.
+#define CU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) \
+	return mb_fail(ctx, e_ == cudaErrorMemoryAllocation ? MB200_ENOMEM : MB200_ECUDA, \
+	  "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
+#define ENSURE(buf, bytes) do { if ((buf).ensure(bytes) != 0) \
+	return mb_fail(ctx, MB200_ENOMEM, "device allocation of %zu bytes failed (%s)", (size_t)(bytes), #buf); } while (0)
 int mb_store_pack_inplace(mb200_ctx *ctx);
 int mb_store_build_transposed(mb200_ctx *ctx);
 int mb_store_refresh_transposed(mb200_ctx *ctx);

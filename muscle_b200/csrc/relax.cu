@@ -35,12 +35,6 @@
 #include <cstdlib>
 #include <cstring>
 
-#define CU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) \
-	return mb_fail(ctx, e_ == cudaErrorMemoryAllocation ? MB200_ENOMEM : MB200_ECUDA, \
-	  "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
-#define ENSURE(buf, bytes) do { if ((buf).ensure(bytes) != 0) \
-	return mb_fail(ctx, MB200_ENOMEM, "device allocation of %zu bytes failed (%s)", (size_t)(bytes), #buf); } while (0)
-
 // ---------------------------------------------------------------------------------------------
 // column bit masks of one orientation.  Rows are addressed like the CSR offsets: slot
 // rowbase[k] + i for row i of store pair k (the slot of the sentinel offset holds an empty row).

@@ -11,12 +11,6 @@
 #include <algorithm>
 #include <cstring>
 
-#define CU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) \
-	return mb_fail(ctx, e_ == cudaErrorMemoryAllocation ? MB200_ENOMEM : MB200_ECUDA, \
-	  "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
-#define ENSURE(buf, bytes) do { if ((buf).ensure(bytes) != 0) \
-	return mb_fail(ctx, MB200_ENOMEM, "device allocation of %zu bytes failed (%s)", (size_t)(bytes), #buf); } while (0)
-
 // ---------------------------------------------------------------------------------------------
 // one warp per pair: copy the pair's entries to their packed position
 __global__ void k_pack_entries(uint32_t npairs, const uint64_t *__restrict__ src_base,

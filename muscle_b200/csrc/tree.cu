@@ -13,12 +13,6 @@
 #include <cfloat>
 #include <cstring>
 
-#define CU(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) \
-	return mb_fail(ctx, e_ == cudaErrorMemoryAllocation ? MB200_ENOMEM : MB200_ECUDA, \
-	  "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
-#define ENSURE(buf, bytes) do { if ((buf).ensure(bytes) != 0) \
-	return mb_fail(ctx, MB200_ENOMEM, "device allocation of %zu bytes failed (%s)", (size_t)(bytes), #buf); } while (0)
-
 #define UP_THREADS 1024
 #define UP_NONE 0xffffffffu
 
