@@ -205,23 +205,24 @@ int mb200_set_hmm(mb200_ctx *ctx, const float start[5], const float trans[25], c
 	if (!ctx || !start || !trans || !ins || !match)
 		return mb_fail(ctx, MB200_EINVAL, "mb200_set_hmm: NULL argument");
 	cudaSetDevice(ctx->device);
-	MbHmm &h = ctx->hmm;
+	// validate before touching the context (a rejected table leaves the previous one in force)
+	int nclass = 0;
+	int rep[256];
+	uint8_t byte2class[256];
+	mb200_residue_classes(ins, match, byte2class, &nclass, rep);
+	if (nclass > MB_MAX_K)
+		return mb_fail(ctx, MB200_EALPHABET, "%d distinct residue classes in the HMM tables, device tables hold %d",
+		  nclass, MB_MAX_K);
+	MbHmm h = ctx->hmm;
 	// state order M=0, IX=1, IY=2, JX=3, JY=4 (pairhmm.h:11-19); aliases of hmmscores.h:1-13
 	h.tSM = start[0]; h.tSI = start[1]; h.tSJ = start[3];
 	h.tMM = trans[0*5 + 0]; h.tMI = trans[0*5 + 1]; h.tMJ = trans[0*5 + 3];
 	h.tII = trans[1*5 + 1]; h.tIM = trans[1*5 + 0];
 	h.tJJ = trans[3*5 + 3]; h.tJM = trans[3*5 + 0];
 	h.minScore = min_sparse_score;
-
-	int nclass = 0;
-	int rep[256];
-	mb200_residue_classes(ins, match, ctx->byte2class, &nclass, rep);
-	if (nclass > MB_MAX_K)
-		return mb_fail(ctx, MB200_EALPHABET, "%d distinct residue classes in the HMM tables, device tables hold %d",
-		  nclass, MB_MAX_K);
 	h.K = nclass;
 	h.KS = nclass | 1;                 // odd row stride spreads match rows over the smem banks
-	h.pad = ctx->byte2class[0];       // the reference reads byte 0 past the sequence end (bwdflat3.cpp:48,66)
+	h.pad = byte2class[0];            // the reference reads byte 0 past the sequence end (bwdflat3.cpp:48,66)
 	std::vector<float> insT(h.K), matchT((size_t) h.K*h.KS, 0.0f);
 	for (int a = 0; a < h.K; ++a)
 		{
@@ -234,6 +235,8 @@ int mb200_set_hmm(mb200_ctx *ctx, const float start[5], const float trans[25], c
 	CU(cudaMemcpyAsync(ctx->d_insT.p, insT.data(), insT.size()*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
 	CU(cudaMemcpyAsync(ctx->d_matchT.p, matchT.data(), matchT.size()*sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
 	CU(cudaStreamSynchronize(ctx->stream));
+	ctx->hmm = h;
+	memcpy(ctx->byte2class, byte2class, sizeof(byte2class));
 	ctx->have_hmm = true;
 	ctx->store_valid = false;
 	if (ctx->nseq > 0)
