@@ -23,10 +23,9 @@
 // and the Backward read are full 128-byte lines.  Backward walks the same anti-diagonals in
 // reverse, fuses the Fwd (*) Bwd posterior score, thresholds it at log(0.01) and appends the scores of
 // survivors to a per-row candidate list; the warp then turns the scores into probabilities 32 at a time,
-// compacts the rows into MySparseMx order and runs the
-// expected-accuracy max-sum DP row by row as a warp-wide prefix-max (new[j] = max_{k<=j}
-// max(old[k], old[k-1]+P[k]) is exactly the reference's max3 recurrence because every value is an
-// exact max of the same sums).
+// compacts the rows into MySparseMx order and runs the expected-accuracy max-sum DP from the candidates
+// through a prefix-max tree over the columns (see mb_compact_ea for why that is exactly the reference's
+// max3 recurrence).
 //
 // Border handling without special code paths: LOG_ZERO is absorbing under the branch-free LogAdd,
 // so the reference's border formulas (first row/column of Forward, fwdflat3.cpp:35-93; last
@@ -207,13 +206,22 @@ __device__ __forceinline__ void mb_stage_y(const MbSeq &Y, int j, int C, int lan
 
 // Compaction and expected accuracy of one pair of a chain, once Backward has left its candidate rows (scores,
 // columns descending) at prow / pcnt: the warp turns the scores into probabilities 32 at a time, writes the
-// entries >= 0.01 in MySparseMx order with their row offsets, and runs the expected-accuracy max-sum DP
-// row by row as a warp-wide prefix-max (new[j] = max_{k<=j} max(old[k], old[k-1]+P[k])), strip by strip
-// through the edge buffers eIn / eOut.  kept: the lane's kept candidates of the pair.
+// entries >= 0.01 in MySparseMx order with their row offsets, and runs the expected-accuracy max-sum DP of
+// CalcAlnScoreFlat (calcalnscoreflat.cpp:4-32).  kept: the lane's kept candidates of the pair.
+//
+// One strip (g.n == 1): from the candidates alone.  A cell without a candidate has P = 0 and fl(x + 0) = x,
+// and rounding is monotone, so fl(max(a, b) + P) = max(fl(a + P), fl(b + P)); the reference's DP therefore
+// computes, for each candidate (i, j), V = fl(P + Q) with Q the max of V over the candidates (i' < i, j' < j)
+// (0 if none), and returns the max of all V (0 if none): bit for bit the same values, with the one addition
+// B = Prevj1 + P it performs.  Q comes from a prefix-max Fenwick tree over the columns in the warp's state
+// area (LY + 1 <= 32*CM words), queried by every candidate of row i before any of row i updates it.
+// Several strips: a warp-wide prefix-max over every column of the row (new[j] = max_{k<=j} max(old[k],
+// old[k-1]+P[k])), strip by strip through the edge buffers eIn / eOut.
 template <bool MEGA, int CM>
 __device__ void mb_compact_ea(const PostParams &P, uint32_t pair, int LX, int LY, uint32_t kept,
   const mb200_entry *prow, const uint8_t *pcnt, const MbStrips &g, float *wbase, float *eIn, float *eOut)
 	{
+	static_assert(32*CM + 32 + 2*MB_CAP <= MB_SM_ARRAYS*CM*32, "the EA tree and a row's updates fit the state area");
 	const int lane = threadIdx.x & 31;
 	const int C = g.C, W = g.W;
 	for (int o = 16; o > 0; o >>= 1)
@@ -234,116 +242,241 @@ __device__ void mb_compact_ea(const PostParams &P, uint32_t pair, int LX, int LY
 	mb200_entry *out = P.entries + base;
 
 	float eaScore = 0.0f;
-	// the warp's state area, reused as three plain float arrays of CM*32
-	float *old = wbase;                 // [c][lane]
-	float *rowbuf = wbase + CM*32;      // column-linear: [lane*C + c]
-	float *pre = wbase + 2*CM*32;       // [c][lane]
 	uint32_t written = 0;
-	for (int strip = 0; strip < g.n; ++strip)
+	if (g.n == 1)
 		{
-		const auto [j0, nl, cn, last] = g.at(strip, lane);
-		for (int c = 0; c < C; ++c)
-			{
-			old[c*32 + lane] = 0.0f;
-			rowbuf[c*32 + lane] = 0.0f;
-			}
+		// node k of the tree (1..LY) holds the max of V over columns k - (k & -k) .. k-1 of the rows done.  The
+		// values are >= +0, so their bits order as integers and an integer max on them is a float max.
+		// Rows are packed: a pack is the next rows whose candidates add up to at most 32 (C3 rows average ~7),
+		// lane k holding row i+k's count and lane l candidate l of the pack, so that the loads, expf and the
+		// compaction run once per pack instead of once per row; only the tree's queries and updates go row by
+		// row.  A row of more than 32 candidates runs alone, batch by batch, its updates held in pend until
+		// all its batches have queried.  The batch code is not shared with the strip path below: that cost the
+		// plain CM = 14 / 16 and the MEGA Backward loops 1 and 3 instructions.
+		float *tree = wbase;
+		uint2 *pend = reinterpret_cast<uint2 *>(wbase + 32*CM + 32);     // a long row's updates: {bits of V, column + 1}
+		for (int k = lane; k <= LY; k += 32)
+			tree[k] = 0.0f;
+		uint32_t vmax = 0;
 		__syncwarp();
-		for (int i = 1; i <= LX; ++i)
+		for (int i = 1; i <= LX; )
 			{
-			const uint32_t cnt = pcnt[i - 1];
-			const mb200_entry *row = prow + (size_t)(i - 1)*MB_CAP;
-			if (strip == 0 && lane == 0)
-				rowoff[i - 1] = written;
-			for (uint32_t e0 = 0; e0 < cnt; e0 += 32)
+			const uint32_t rc = i + lane <= LX ? pcnt[i - 1 + lane] : 0u;
+			uint32_t incl = rc;
+#pragma unroll
+			for (int o = 1; o < 32; o <<= 1)
 				{
-				const int idx = (int) cnt - 1 - (int)(e0 + lane);
-				mb200_entry ent; ent.p = 0.0f; ent.col = 0;
-				if (idx >= 0)
+				const uint32_t n = __shfl_up_sync(MB_FULL, incl, o);
+				if (lane >= o)
+					incl += n;
+				}
+			const uint32_t excl = incl - rc;
+			const int m = max(1, __popc(__ballot_sync(MB_FULL, incl <= 32u && i + lane <= LX)));
+			const uint32_t cnt0 = __shfl_sync(MB_FULL, rc, 0);
+			if (cnt0 > 32u)
+				{
+				// a row of more than 32 candidates on its own, batch by batch
+				const mb200_entry *row = prow + (size_t)(i - 1)*MB_CAP;
+				if (lane == 0)
+					rowoff[i - 1] = written;
+				for (uint32_t e0 = 0; e0 < cnt0; e0 += 32)
 					{
-					ent = row[idx];             // {score, column}: the probability (calcposteriorflat.cpp:20)
-					ent.p = ent.p >= 0.0f ? 1.0f : mb_expf_glibc(ent.p);
-					}
-				const int lc = (int) ent.col - j0;
-				if (idx >= 0 && lc >= 0 && lc < W)
-					rowbuf[lc] = ent.p;
-				if (strip == 0)
-					{
+					const int idx = (int) cnt0 - 1 - (int)(e0 + lane);
+					mb200_entry ent; ent.p = 0.0f; ent.col = 0;
+					if (idx >= 0)
+						{
+						ent = row[idx];             // {score, column}: the probability (calcposteriorflat.cpp:20)
+						ent.p = ent.p >= 0.0f ? 1.0f : mb_expf_glibc(ent.p);
+						}
 					const bool keep = idx >= 0 && ent.p >= 0.01f;          // mysparsemx.cpp:139-141
 					const uint32_t b = __ballot_sync(MB_FULL, keep);
 					if (keep && fits)
 						out[written + __popc(b & ((1u << lane) - 1u))] = ent;
 					written += __popc(b);
+					if (idx >= 0)
+						{
+						float q = 0.0f;
+						for (uint32_t k = ent.col; k > 0; k &= k - 1)
+							q = fmaxf(q, tree[k]);
+						const uint32_t v = __float_as_uint(ADD(ent.p, q));
+						vmax = max(vmax, v);
+						pend[e0 + lane] = make_uint2(v, ent.col + 1);
+						}
 					}
-				}
-			__syncwarp();
-			// calcalnscoreflat.cpp:13-29 as a prefix-max over the row
-			float leftOld = 0.0f, incoming = 0.0f;
-			if (lane == 0)
-				{
-				leftOld = strip == 0 ? 0.0f : eIn[i - 1];
-				incoming = strip == 0 ? 0.0f : eIn[i];
-				}
-			else
-				leftOld = old[(C - 1)*32 + lane - 1];
-			float run = 0.0f, prevOld = leftOld;
-			for (int c = 0; c < C; ++c)
-				{
-				const float o = old[c*32 + lane];
-				const float b = ADD(prevOld, rowbuf[lane*C + c]);
-				float v = fmaxf(o, b);
-				v = c == 0 ? v : fmaxf(v, run);
-				run = v;
-				pre[c*32 + lane] = v;
-				prevOld = o;
-				}
-			__syncwarp();
-			float scan = run;
-#pragma unroll
-			for (int o = 1; o < 32; o <<= 1)
-				{
-				const float n = __shfl_up_sync(MB_FULL, scan, o);
-				if (lane >= o)
-					scan = fmaxf(scan, n);
-				}
-			float excl = __shfl_up_sync(MB_FULL, scan, 1);
-			const float inc0 = __shfl_sync(MB_FULL, incoming, 0);
-			excl = lane == 0 ? inc0 : fmaxf(excl, inc0);
-			float lastNew = 0.0f;
-			for (int c = 0; c < C; ++c)
-				{
-				lastNew = fmaxf(pre[c*32 + lane], excl);
-				old[c*32 + lane] = lastNew;
-				}
-			if (lane == 31 && !last)
-				eOut[i] = lastNew;
-			__syncwarp();
-			for (uint32_t e0 = 0; e0 < cnt; e0 += 32)
-				{
-				const int idx = (int) cnt - 1 - (int)(e0 + lane);
-				if (idx >= 0)
+				__syncwarp();
+				for (uint32_t e = lane; e < cnt0; e += 32)
 					{
-					const int lc = (int) row[idx].col - j0;
-					if (lc >= 0 && lc < W)
-						rowbuf[lc] = 0.0f;
+					const uint2 u = pend[e];
+					for (uint32_t k = u.y; k <= (uint32_t) LY; k += k & (0u - k))
+						atomicMax(reinterpret_cast<int *>(tree) + k, (int) u.x);
 					}
+				__syncwarp();
+				++i;
+				continue;
+				}
+			// the pack's row r of lane l: the number of rows k < m with incl[k] <= l; candidate l - excl[r] of it
+			// in ascending column order
+			int r = 0;
+#pragma unroll
+			for (int o = 16; o > 0; o >>= 1)
+				{
+				const uint32_t t = __shfl_sync(MB_FULL, incl, min(r + o - 1, 31));
+				if (r + o <= m && t <= (uint32_t) lane)
+					r += o;
+				}
+			const uint32_t total = __shfl_sync(MB_FULL, incl, m - 1);
+			const bool has = (uint32_t) lane < total;
+			const uint32_t rcnt = __shfl_sync(MB_FULL, rc, r), rex = __shfl_sync(MB_FULL, excl, r);
+			mb200_entry ent; ent.p = 0.0f; ent.col = 0;
+			if (has)
+				{
+				ent = prow[(size_t)(i - 1 + r)*MB_CAP + rcnt - 1 - (lane - rex)];
+				ent.p = ent.p >= 0.0f ? 1.0f : mb_expf_glibc(ent.p);
+				}
+			const bool keep = has && ent.p >= 0.01f;
+			const uint32_t b = __ballot_sync(MB_FULL, keep);
+			if (keep && fits)
+				out[written + __popc(b & ((1u << lane) - 1u))] = ent;
+			if (lane < m)
+				rowoff[i - 1 + lane] = written + __popc(excl < 32u ? b & ((1u << excl) - 1u) : b);
+			written += __popc(b);
+			// the tree row by row: a row's queries see the rows before it only
+			for (int k = 0; k < m; ++k)
+				{
+				const bool mine = has && r == k;
+				uint32_t v = 0;
+				if (mine)
+					{
+					float q = 0.0f;
+					for (uint32_t t = ent.col; t > 0; t &= t - 1)
+						q = fmaxf(q, tree[t]);
+					v = __float_as_uint(ADD(ent.p, q));
+					vmax = max(vmax, v);
+					}
+				__syncwarp();
+				if (mine)
+					for (uint32_t t = ent.col + 1; t <= (uint32_t) LY; t += t & (0u - t))
+						atomicMax(reinterpret_cast<int *>(tree) + t, (int) v);
+				__syncwarp();
+				}
+			i += m;
+			}
+		if (lane == 0)
+			rowoff[LX] = written;
+		eaScore = __uint_as_float(__reduce_max_sync(MB_FULL, vmax));
+		}
+	else
+		{
+		// the warp's state area, reused as three plain float arrays of CM*32
+		float *old = wbase;                 // [c][lane]
+		float *rowbuf = wbase + CM*32;      // column-linear: [lane*C + c]
+		float *pre = wbase + 2*CM*32;       // [c][lane]
+		for (int strip = 0; strip < g.n; ++strip)
+			{
+			const auto [j0, nl, cn, last] = g.at(strip, lane);
+			for (int c = 0; c < C; ++c)
+				{
+				old[c*32 + lane] = 0.0f;
+				rowbuf[c*32 + lane] = 0.0f;
 				}
 			__syncwarp();
+			for (int i = 1; i <= LX; ++i)
+				{
+				const uint32_t cnt = pcnt[i - 1];
+				const mb200_entry *row = prow + (size_t)(i - 1)*MB_CAP;
+				if (strip == 0 && lane == 0)
+					rowoff[i - 1] = written;
+				for (uint32_t e0 = 0; e0 < cnt; e0 += 32)
+					{
+					const int idx = (int) cnt - 1 - (int)(e0 + lane);
+					mb200_entry ent; ent.p = 0.0f; ent.col = 0;
+					if (idx >= 0)
+						{
+						ent = row[idx];             // {score, column}: the probability (calcposteriorflat.cpp:20)
+						ent.p = ent.p >= 0.0f ? 1.0f : mb_expf_glibc(ent.p);
+						}
+					const int lc = (int) ent.col - j0;
+					if (idx >= 0 && lc >= 0 && lc < W)
+						rowbuf[lc] = ent.p;
+					if (strip == 0)
+						{
+						const bool keep = idx >= 0 && ent.p >= 0.01f;          // mysparsemx.cpp:139-141
+						const uint32_t b = __ballot_sync(MB_FULL, keep);
+						if (keep && fits)
+							out[written + __popc(b & ((1u << lane) - 1u))] = ent;
+						written += __popc(b);
+						}
+					}
+				__syncwarp();
+				// calcalnscoreflat.cpp:13-29 as a prefix-max over the row
+				float leftOld = 0.0f, incoming = 0.0f;
+				if (lane == 0)
+					{
+					leftOld = strip == 0 ? 0.0f : eIn[i - 1];
+					incoming = strip == 0 ? 0.0f : eIn[i];
+					}
+				else
+					leftOld = old[(C - 1)*32 + lane - 1];
+				float run = 0.0f, prevOld = leftOld;
+				for (int c = 0; c < C; ++c)
+					{
+					const float o = old[c*32 + lane];
+					const float b = ADD(prevOld, rowbuf[lane*C + c]);
+					float v = fmaxf(o, b);
+					v = c == 0 ? v : fmaxf(v, run);
+					run = v;
+					pre[c*32 + lane] = v;
+					prevOld = o;
+					}
+				__syncwarp();
+				float scan = run;
+#pragma unroll
+				for (int o = 1; o < 32; o <<= 1)
+					{
+					const float n = __shfl_up_sync(MB_FULL, scan, o);
+					if (lane >= o)
+						scan = fmaxf(scan, n);
+					}
+				float excl = __shfl_up_sync(MB_FULL, scan, 1);
+				const float inc0 = __shfl_sync(MB_FULL, incoming, 0);
+				excl = lane == 0 ? inc0 : fmaxf(excl, inc0);
+				float lastNew = 0.0f;
+				for (int c = 0; c < C; ++c)
+					{
+					lastNew = fmaxf(pre[c*32 + lane], excl);
+					old[c*32 + lane] = lastNew;
+					}
+				if (lane == 31 && !last)
+					eOut[i] = lastNew;
+				__syncwarp();
+				for (uint32_t e0 = 0; e0 < cnt; e0 += 32)
+					{
+					const int idx = (int) cnt - 1 - (int)(e0 + lane);
+					if (idx >= 0)
+						{
+						const int lc = (int) row[idx].col - j0;
+						if (lc >= 0 && lc < W)
+							rowbuf[lc] = 0.0f;
+						}
+					}
+				__syncwarp();
+				}
+			if (strip == 0 && lane == 0)
+				rowoff[LX] = written;
+			if (lane == 31 && !last)
+				eOut[0] = 0.0f;
+			if (last)
+				{
+				// cell (LX,LY), local column g.clast of lane g.lcl.  Which form ptxas compiles best differs by mode:
+				// reading g.clast keeps it live through Backward and costs the plain CM = 14 and 16 kernels a
+				// register and 2 instructions per Backward column; forming the cell from LY instead costs the
+				// MEGA kernels 2 instructions per Backward column.
+				const int q = LY - 1 - j0;
+				eaScore = MEGA ? old[g.clast*32 + g.lcl] : old[(q % C)*32 + q/C];
+				}
+			__syncwarp();
+			float *tmp = eIn; eIn = eOut; eOut = tmp;
 			}
-		if (strip == 0 && lane == 0)
-			rowoff[LX] = written;
-		if (lane == 31 && !last)
-			eOut[0] = 0.0f;
-		if (last)
-			{
-			// cell (LX,LY), local column g.clast of lane g.lcl.  Which form ptxas compiles best differs by mode:
-			// reading g.clast keeps it live through Backward and costs the plain CM = 14 and 16 kernels a
-			// register and 2 instructions per Backward column; forming the cell from LY instead costs the
-			// MEGA kernels 2 instructions per Backward column.
-			const int q = LY - 1 - j0;
-			eaScore = MEGA ? old[g.clast*32 + g.lcl] : old[(q % C)*32 + q/C];
-			}
-		__syncwarp();
-		float *tmp = eIn; eIn = eOut; eOut = tmp;
 		}
 	if (lane == 0)
 		P.ea[pair] = __fdiv_rn(eaScore, (float) min(LX, LY));     // calcposteriorflat.cpp:89
