@@ -1399,15 +1399,21 @@ static int buildpost_by_cell(mb200_ctx *ctx, const BuildPostParams &P, const uin
 		}
 	return MB200_OK;
 	}
+// Shared memory of one k_bp_apply block: the accumulator rows of BP_WARPS warps + their cp.async buffers.
+// The ordered row walk runs only where this fits (cols_b <= 12544).
+#define BP_SMEM_MAX (220*1024)
+static size_t bp_row_smem(uint32_t cols_b)
+	{
+	return (((size_t) BP_WARPS*cols_b*sizeof(float) + 15) & ~(size_t) 15) + (size_t) BP_WARPS*BP_NBUF*BP_G*BP_W*sizeof(uint2);
+	}
 // BuildPost as an ordered walk over the rows (k_bp_gather / k_bp_apply).  Scratch: d_stage, d_tmp2.  No read-backs.
 static int buildpost_by_row(mb200_ctx *ctx, const BuildPostParams &P, const uint32_t *d_rb, const std::vector<uint32_t> &h_rb,
   const MemberBatches &bt, JoinTimer &T)
 	{
 	cudaStream_t st = ctx->stream;
 	const uint32_t cols_a = P.cols_a;
-	// the accumulator rows of BP_WARPS warps + their cp.async double buffers must fit in shared memory
-	const size_t acc_smem = (((size_t) BP_WARPS*P.cols_b*sizeof(float) + 15) & ~(size_t) 15) + (size_t) BP_WARPS*BP_NBUF*BP_G*BP_W*sizeof(uint2);
-	if (acc_smem > 220*1024)
+	const size_t acc_smem = bp_row_smem(P.cols_b);
+	if (acc_smem > BP_SMEM_MAX)
 		return mb_fail(ctx, MB200_EOVERFLOW, "alignment with %u columns too wide for the BuildPost kernel", P.cols_b);
 	ENSURE(ctx->d_stage, bt.max_rows*BP_W*sizeof(uint2) + 256);
 	BpStage G;
@@ -1488,7 +1494,9 @@ static int join_core(mb200_ctx *ctx, const JoinMembers &M, uint32_t cols_a, uint
 		++colbits;
 	while ((1u << rowbits) < cols_a)
 		++rowbits;
-	const bool by_cell = (uint64_t) M.h_rb[na]*nb >= (uint64_t) sort_min && colbits + rowbits <= 32 && na <= 65535;
+	// a join too wide for the row walk's shared-memory accumulator takes the by-cell route whatever its size
+	const bool by_cell = ((uint64_t) M.h_rb[na]*nb >= (uint64_t) sort_min || bp_row_smem(cols_b) > BP_SMEM_MAX)
+	  && colbits + rowbits <= 32 && na <= 65535;
 	// batches of A's members: by cell at most ~16M (residue, t) rows; by row, the staging area (one slot
 	// per residue of the batch and member of B) stays below ~2 GB
 	const MemberBatches bt = member_batches(M.h_rb, nb, by_cell ? 16ull << 20 : (2048ull << 20)/(BP_W*sizeof(uint2)));
