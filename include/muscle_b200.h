@@ -247,7 +247,9 @@ int mb200_calc_post_dense_pair(mb200_ctx *ctx, uint32_t npairs, const uint32_t *
  * that every device ends with the complete store; mb200_group_consistency_iter replaces
  * MPCFlat::ConsIter (consflat.cpp:5-23) with every device updating its own pair range followed by an
  * in-place exchange of the updated entries.  The serial stages (mb200_align_groups, mb200_msa_*)
- * run on mb200_group_ctx(g, 0).  devices == NULL or ndev <= 0: all visible devices. */
+ * run on mb200_group_ctx(g, 0).  devices == NULL: the first ndev visible devices (all if ndev <= 0),
+ * or, when the environment sets MB200_DEVICE_LIST=a,b,..., one member per listed device; a list may
+ * repeat a device (several members on one GPU).  devices != NULL and ndev <= 0: all visible devices. */
 typedef struct mb200_group mb200_group;
 int         mb200_group_create(int ndev, const int *devices, mb200_group **out);
 void        mb200_group_destroy(mb200_group *g);

@@ -69,7 +69,8 @@ static void EnsureGroup()
 	{
 	if (g_Group != 0)
 		return;
-	// MB200_DEVICES=n: use the first n visible GPUs (default: all); MB200_DEVICE=d: only device d
+	// MB200_DEVICES=n: use the first n visible GPUs (default: all); MB200_DEVICE=d: only device d.
+	// Without MB200_DEVICE the library reads MB200_DEVICE_LIST=a,b,... itself (mb200_group_create).
 	int rc;
 	const char *one = getenv("MB200_DEVICE");
 	const char *cnt = getenv("MB200_DEVICES");

@@ -17,6 +17,7 @@
 #include <chrono>
 #include <cstdarg>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <thread>
 #include <vector>
@@ -70,6 +71,25 @@ static int on_all(mb200_group *g, F f)
 	return MB200_OK;
 	}
 
+// "a,b,..." -> device numbers; false unless the whole string is a non-empty comma-separated list
+static bool parse_device_list(const char *s, std::vector<int> &out)
+	{
+	out.clear();
+	for (const char *p = s;;)
+		{
+		char *end = nullptr;
+		const long d = strtol(p, &end, 10);
+		if (end == p || d < 0 || d > 4096)
+			return false;
+		out.push_back((int) d);
+		if (*end == 0)
+			return true;
+		if (*end != ',')
+			return false;
+		p = end + 1;
+		}
+	}
+
 extern "C" {
 
 const char *mb200_group_last_error(const mb200_group *g) { return g ? g->err : g_group_create_error; }
@@ -86,7 +106,16 @@ int mb200_group_create(int ndev, const int *devices, mb200_group **out)
 		return gfail(nullptr, MB200_ENODEV, "no CUDA device; libmuscle_b200 has no CPU path");
 		}
 	std::vector<int> devs;
-	if (ndev <= 0 || devices == nullptr)
+	// MB200_DEVICE_LIST=a,b,...: the members of a group whose caller leaves the devices to the library,
+	// one per listed device.  Repeats are allowed: every member is its own context, and a same-device peer
+	// copy is a device-to-device copy, so a list like 0,0,0 runs the sharded path on one GPU.
+	const char *list = devices == nullptr ? getenv("MB200_DEVICE_LIST") : nullptr;
+	if (list != nullptr)
+		{
+		if (!parse_device_list(list, devs))
+			return gfail(nullptr, MB200_EINVAL, "MB200_DEVICE_LIST=%s: expected comma-separated device numbers", list);
+		}
+	else if (ndev <= 0 || devices == nullptr)
 		{
 		const int n = ndev <= 0 ? have : std::min(ndev, have);
 		for (int d = 0; d < n; ++d)

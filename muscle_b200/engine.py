@@ -423,6 +423,21 @@ class Group:
 		self.nseq = len(bs)
 		self._ck(self.lib.mb200_group_set_seqs(self.g, C.c_uint32(len(bs)), _ptr(buf), _ptr(off)))
 
+	def set_seqs_mega(self, model, profiles):
+		"""Mega feature profiles on every member: the arguments of Engine.set_seqs_mega"""
+		F = len(model["alpha"])
+		alpha = np.ascontiguousarray(model["alpha"], np.uint32)
+		w = np.ascontiguousarray(model["weights"], np.float32)
+		lp = np.ascontiguousarray(model["logprobs"], np.float32)
+		lpm = np.ascontiguousarray(model["logprobmx"], np.float32)
+		self.lens = np.array([len(p) for p in profiles], np.int64)
+		off = np.zeros(len(profiles) + 1, np.uint64)
+		off[1:] = np.cumsum(self.lens)
+		let = np.ascontiguousarray(np.concatenate([np.asarray(p, np.uint8).reshape(-1, F) for p in profiles]), np.uint8)
+		self.nseq = len(profiles)
+		self._ck(self.lib.mb200_group_set_seqs_mega(self.g, C.c_uint32(self.nseq), _ptr(let), _ptr(off), C.c_uint32(F),
+		  _ptr(alpha), _ptr(w), _ptr(lp), _ptr(lpm)))
+
 	def posteriors_allpairs(self, want_ea=True):
 		n = self.nseq
 		ea = np.empty(n*(n - 1)//2, np.float32) if want_ea else None
