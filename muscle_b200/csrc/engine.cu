@@ -699,6 +699,7 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 	ctx->store_tr_valid = false;
 	ctx->store_masks_valid = false;
 	ctx->store_packed = false;
+	ctx->h_index_valid = false;            // the device now holds another nnz / entbase index
 	return MB200_OK;
 	}
 
@@ -910,7 +911,8 @@ int mb200_export_pair(mb200_ctx *ctx, uint32_t pair, uint32_t *offsets, mb200_en
 	if (!ctx || !offsets)
 		return mb_fail(ctx, MB200_EINVAL, "mb200_export_pair: bad argument");
 	cudaSetDevice(ctx->device);
-	ctx->h_index_valid = false;
+	// the host index is re-read only when the store changed: at C3 it is 6 MB, and callers export
+	// pairs one at a time
 	int rc = fetch_store_index(ctx);
 	if (rc != MB200_OK)
 		return rc;
