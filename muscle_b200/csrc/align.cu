@@ -486,12 +486,12 @@ __device__ __forceinline__ void bp_operand(const BuildPostParams &P, uint32_t a,
 	{
 	if (a < b)
 		{
-		const uint32_t q = (uint32_t)((uint64_t) a*P.n - (uint64_t) a*(a + 1)/2 + (b - a - 1));
+		const uint32_t q = mb_pair_index(P.n, a, b);
 		ro = P.rowoff + P.rowbase[q]; en = P.entries + P.entbase[q];
 		}
 	else
 		{
-		const uint32_t q = (uint32_t)((uint64_t) b*P.n - (uint64_t) b*(b + 1)/2 + (a - b - 1));
+		const uint32_t q = mb_pair_index(P.n, b, a);
 		ro = P.troff + P.trbase[q]; en = P.trentries + P.entbase[q];
 		}
 	}
@@ -946,14 +946,14 @@ __global__ void k_bpc_count(const BuildPostParams P, const BpCells G)
 		uint64_t ep;
 		if (a < b)
 			{
-			const uint32_t q = (uint32_t)((uint64_t) a*P.n - (uint64_t) a*(a + 1)/2 + (b - a - 1));
+			const uint32_t q = mb_pair_index(P.n, a, b);
 			const uint32_t *ro = P.rowoff + P.rowbase[q];
 			e0 = ro[pos]; e1 = ro[pos + 1];
 			ep = P.entbase[q] + e0;
 			}
 		else
 			{
-			const uint32_t q = (uint32_t)((uint64_t) b*P.n - (uint64_t) b*(b + 1)/2 + (a - b - 1));
+			const uint32_t q = mb_pair_index(P.n, b, a);
 			const uint32_t *ro = P.troff + P.trbase[q];
 			e0 = ro[pos]; e1 = ro[pos + 1];
 			ep = (P.entbase[q] + e0) | (1ull << 63);
@@ -1187,18 +1187,9 @@ struct JoinMembers
 static int join_members(mb200_ctx *ctx, const char *who, uint32_t na, const uint32_t *ids_a, uint32_t nb, const uint32_t *ids_b,
   JoinMembers &M)
 	{
-	if (!ctx->store_valid || !ctx->store_allpairs)
-		return mb_fail(ctx, MB200_EINVAL, "%s: the store must hold all N(N-1)/2 pairs", who);
-	int rc = mb_store_build_transposed(ctx);
+	const int rc = mb_store_require(ctx, who, NEED_ALLPAIRS | FORM_TRANSPOSED);
 	if (rc != MB200_OK)
 		return rc;
-	if (ctx->tr_values_stale)
-		{
-		rc = mb_store_refresh_transposed(ctx);
-		if (rc != MB200_OK)
-			return rc;
-		ctx->tr_values_stale = false;
-		}
 	M.na = na; M.nb = nb;
 	M.ids.resize(na + nb);
 	M.h_rb.assign(na + 1, 0);
@@ -1532,7 +1523,7 @@ int mb200_align_pairs(mb200_ctx *ctx, uint32_t n, const uint32_t *store_pairs, c
 	{
 	if (!ctx || n == 0 || !store_pairs || !paths_out || !path_off || !scores_out)
 		return mb_fail(ctx, MB200_EINVAL, "mb200_align_pairs: bad argument");
-	int rc = mb_store_pack_inplace(ctx);
+	int rc = mb_store_require(ctx, "mb200_align_pairs", FORM_PACKED);
 	if (rc != MB200_OK)
 		return rc;
 	cudaSetDevice(ctx->device);
@@ -1583,7 +1574,9 @@ int mb200_align_pairs(mb200_ctx *ctx, uint32_t n, const uint32_t *store_pairs, c
 		q.plen = nullptr;
 		DensifyJob &j = jobs[k];
 		j.rowoff = (const uint32_t *) ctx->d_rowoff.p + ctx->h_rowbase[sp];
-		j.entries = (const mb200_entry *) ctx->d_entries.p + ctx->h_entbase[sp];
+		uint64_t e_lo = 0, e_hi = 0;
+		mb_store_entry_range(ctx, sp, sp + 1, &e_lo, &e_hi);
+		j.entries = (const mb200_entry *) ctx->d_entries.p + e_lo;
 		j.dense = (float *) q.dense;
 		j.LX = L.LX; j.ld = L.ld;
 		od += al256(L.dense_bytes);

@@ -19,6 +19,12 @@
 #define MB_CHAIN_MAX 32                 // posterior kernel: pairs in one chain (one per lane when the chain is read)
 #define MB_CHAIN_BUF (MB_CHAIN_MAX*38)  // words of per-warp chain scratch: kept counts [pair][lane], totals [pair], final cells [pair][5]
 
+// index of pair (a,b), a < b, in the row-major all-pairs order of the store (mpcflat.cpp:139-159)
+__host__ __device__ __forceinline__ uint32_t mb_pair_index(uint32_t n, uint32_t a, uint32_t b)
+	{
+	return (uint32_t)((uint64_t) a*n - (uint64_t) a*(a + 1)/2 + (b - a - 1));
+	}
+
 struct MbHmm
 	{
 	float tSM, tSI, tSJ, tMM, tMI, tMJ, tII, tIM, tJJ, tJM;   // hmmscores.h:1-13

@@ -238,7 +238,7 @@ int mb200_set_hmm(mb200_ctx *ctx, const float start[5], const float trans[25], c
 	ctx->hmm = h;
 	memcpy(ctx->byte2class, byte2class, sizeof(byte2class));
 	ctx->have_hmm = true;
-	ctx->store_valid = false;
+	mb_store_drop(ctx);
 	if (ctx->nseq > 0)
 		return recode_seqs(ctx);
 	return MB200_OK;
@@ -258,41 +258,56 @@ static int recode_seqs(mb200_ctx *ctx)
 	return MB200_OK;
 	}
 
+// Offsets of mb200_set_seqs / mb200_set_seqs_mega: every sequence non-empty and shorter than 2^31
+static int check_offsets(mb200_ctx *ctx, uint32_t nseq, const uint64_t *offsets, const char *what)
+	{
+	for (uint32_t i = 0; i < nseq; ++i)
+		{
+		if (offsets[i + 1] <= offsets[i])
+			return mb_fail(ctx, MB200_EINVAL, "%s %u is empty or offsets not increasing", what, i);
+		if (offsets[i + 1] - offsets[i] > 0x7fffffffull)
+			return mb_fail(ctx, MB200_EOVERFLOW, "%s %u too long", what, i);
+		}
+	return MB200_OK;
+	}
+
+// New sequences of either kind, validated: offsets from 0 and lengths on host and device, the statistics
+// restart, and the pair list, the store and the MSAs of the old ones are dropped.  Enqueues uploads only.
+static int install_seqs(mb200_ctx *ctx, uint32_t nseq, const uint64_t *offsets, bool mega)
+	{
+	ctx->nseq = nseq;
+	ctx->mega = mega;
+	ctx->h_off.assign(offsets, offsets + nseq + 1);
+	for (auto &o : ctx->h_off)
+		o -= offsets[0];
+	ctx->h_len.resize(nseq);
+	for (uint32_t i = 0; i < nseq; ++i)
+		ctx->h_len[i] = (uint32_t)(offsets[i + 1] - offsets[i]);
+	ctx->msa_valid = false;
+	ENSURE(ctx->d_seqoff, (nseq + 1)*sizeof(uint64_t));
+	ENSURE(ctx->d_seqlen, nseq*sizeof(uint32_t));
+	CU(cudaMemcpyAsync(ctx->d_seqoff.p, ctx->h_off.data(), (nseq + 1)*sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
+	CU(cudaMemcpyAsync(ctx->d_seqlen.p, ctx->h_len.data(), nseq*sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
+	ctx->stats.h2d_bytes = (nseq + 1)*sizeof(uint64_t) + nseq*sizeof(uint32_t);
+	ctx->stats.d2h_bytes = 0;
+	mb_store_set_pairs(ctx, PAIRS_NONE);
+	ctx->last_used_entries = 0;
+	return MB200_OK;
+	}
+
 int mb200_set_seqs(mb200_ctx *ctx, uint32_t nseq, const uint8_t *bytes, const uint64_t *offsets)
 	{
 	if (!ctx || !bytes || !offsets || nseq == 0)
 		return mb_fail(ctx, MB200_EINVAL, "mb200_set_seqs: bad argument");
 	cudaSetDevice(ctx->device);
 	// validate before touching the context (a failed call leaves the previous sequences usable)
-	for (uint32_t i = 0; i < nseq; ++i)
-		{
-		if (offsets[i + 1] <= offsets[i])
-			return mb_fail(ctx, MB200_EINVAL, "sequence %u is empty or offsets not increasing", i);
-		if (offsets[i + 1] - offsets[i] > 0x7fffffffull)
-			return mb_fail(ctx, MB200_EOVERFLOW, "sequence %u too long", i);
-		}
-	ctx->nseq = nseq;
-	ctx->mega = false;
-	ctx->h_off.assign(offsets, offsets + nseq + 1);
-	ctx->h_len.resize(nseq);
-	for (uint32_t i = 0; i < nseq; ++i)
-		ctx->h_len[i] = (uint32_t)(offsets[i + 1] - offsets[i]);
-	ctx->msa_valid = false;
+	int rc = check_offsets(ctx, nseq, offsets, "sequence");
+	if (rc != MB200_OK)
+		return rc;
 	ctx->h_bytes.assign(bytes + offsets[0], bytes + offsets[nseq]);
-	const uint64_t o0 = offsets[0];
-	for (auto &o : ctx->h_off)
-		o -= o0;
-	ENSURE(ctx->d_seqoff, (nseq + 1)*sizeof(uint64_t));
-	ENSURE(ctx->d_seqlen, nseq*sizeof(uint32_t));
-	CU(cudaMemcpyAsync(ctx->d_seqoff.p, ctx->h_off.data(), (nseq + 1)*sizeof(uint64_t), cudaMemcpyHostToDevice, ctx->stream));
-	CU(cudaMemcpyAsync(ctx->d_seqlen.p, ctx->h_len.data(), nseq*sizeof(uint32_t), cudaMemcpyHostToDevice, ctx->stream));
-	ctx->stats.h2d_bytes = (nseq + 1)*sizeof(uint64_t) + nseq*sizeof(uint32_t);   // counters restart at set_seqs
-	ctx->stats.d2h_bytes = 0;
-	ctx->store_valid = false;
-	ctx->store_allpairs = false;
-	ctx->ea_allpairs = false;
-	ctx->plan_valid = false;
-	ctx->last_used_entries = 0;
+	rc = install_seqs(ctx, nseq, offsets, false);
+	if (rc != MB200_OK)
+		return rc;
 	if (ctx->have_hmm)
 		return recode_seqs(ctx);
 	CU(cudaStreamSynchronize(ctx->stream));
@@ -322,13 +337,9 @@ int mb200_set_seqs_mega(mb200_ctx *ctx, uint32_t nseq, const uint8_t *letters, c
 		}
 	if (tsize > 12*1024)
 		return mb_fail(ctx, MB200_EALPHABET, "mb200_set_seqs_mega: pair tables of %u floats do not fit the kernel's shared memory", tsize);
-	for (uint32_t i = 0; i < nseq; ++i)
-		{
-		if (offsets[i + 1] <= offsets[i])
-			return mb_fail(ctx, MB200_EINVAL, "profile %u is empty or offsets not increasing", i);
-		if (offsets[i + 1] - offsets[i] > 0x7fffffffull)
-			return mb_fail(ctx, MB200_EOVERFLOW, "profile %u too long", i);
-		}
+	int rc = check_offsets(ctx, nseq, offsets, "profile");
+	if (rc != MB200_OK)
+		return rc;
 	const uint64_t o0 = offsets[0], npos = offsets[nseq] - o0;
 	std::vector<uint8_t> packed(npos*8, 0);
 	std::vector<float> insP(npos);
@@ -351,8 +362,6 @@ int mb200_set_seqs_mega(mb200_ctx *ctx, uint32_t nseq, const uint8_t *letters, c
 	for (uint32_t f = 0; f < nfeat; ++f)
 		for (uint32_t k = 0; k < alpha[f]*alpha[f]; ++k)
 			T[base[f] + k] = logprobmx[base[f] + k]*weights[f];                 // mega.cpp:355-356
-	ctx->nseq = nseq;
-	ctx->mega = true;
 	ctx->mega_nf = nfeat;
 	ctx->mega_tsize = tsize;
 	for (uint32_t f = 0; f < 8; ++f)
@@ -360,33 +369,19 @@ int mb200_set_seqs_mega(mb200_ctx *ctx, uint32_t nseq, const uint8_t *letters, c
 		ctx->mega_base[f] = f < nfeat ? base[f] : 0;
 		ctx->mega_alpha[f] = f < nfeat ? alpha[f] : 0;
 		}
-	ctx->h_off.assign(offsets, offsets + nseq + 1);
-	for (auto &o : ctx->h_off)
-		o -= o0;
-	ctx->h_len.resize(nseq);
-	for (uint32_t i = 0; i < nseq; ++i)
-		ctx->h_len[i] = (uint32_t)(offsets[i + 1] - offsets[i]);
 	ctx->h_bytes.clear();
-	ctx->msa_valid = false;
-	ENSURE(ctx->d_seqoff, (nseq + 1)*sizeof(uint64_t));
-	ENSURE(ctx->d_seqlen, nseq*sizeof(uint32_t));
+	rc = install_seqs(ctx, nseq, offsets, true);
+	if (rc != MB200_OK)
+		return rc;
 	ENSURE(ctx->d_codes, packed.size() + 16);
 	ENSURE(ctx->d_insP, insP.size()*sizeof(float) + 16);
 	ENSURE(ctx->d_megaT, T.size()*sizeof(float) + 16);
 	cudaStream_t st = ctx->stream;
-	CU(cudaMemcpyAsync(ctx->d_seqoff.p, ctx->h_off.data(), (nseq + 1)*sizeof(uint64_t), cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(ctx->d_seqlen.p, ctx->h_len.data(), nseq*sizeof(uint32_t), cudaMemcpyHostToDevice, st));
 	CU(cudaMemcpyAsync(ctx->d_codes.p, packed.data(), packed.size(), cudaMemcpyHostToDevice, st));
 	CU(cudaMemcpyAsync(ctx->d_insP.p, insP.data(), insP.size()*sizeof(float), cudaMemcpyHostToDevice, st));
 	CU(cudaMemcpyAsync(ctx->d_megaT.p, T.data(), T.size()*sizeof(float), cudaMemcpyHostToDevice, st));
 	CU(cudaStreamSynchronize(st));
-	ctx->stats.h2d_bytes = (nseq + 1)*sizeof(uint64_t) + nseq*sizeof(uint32_t) + packed.size() + insP.size()*4 + T.size()*4;
-	ctx->stats.d2h_bytes = 0;
-	ctx->store_valid = false;
-	ctx->store_allpairs = false;
-	ctx->ea_allpairs = false;
-	ctx->plan_valid = false;
-	ctx->last_used_entries = 0;
+	ctx->stats.h2d_bytes += packed.size() + insP.size()*4 + T.size()*4;
 	return MB200_OK;
 	}
 
@@ -695,11 +690,7 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 	CU(cudaStreamSynchronize(st));
 	cudaEventElapsedTime(&ctx->stats.last_kernel_ms, ctx->ev1, ctx->ev2);
 	cudaEventElapsedTime(&ctx->stats.last_total_ms, ctx->ev0, ctx->ev3);
-	ctx->store_valid = true;
-	ctx->store_tr_valid = false;
-	ctx->store_masks_valid = false;
-	ctx->store_packed = false;
-	ctx->h_index_valid = false;            // the device now holds another nnz / entbase index
+	mb_store_fresh(ctx, false);
 	return MB200_OK;
 	}
 
@@ -708,11 +699,7 @@ static void install_pairs(mb200_ctx *ctx, uint32_t npairs, const uint32_t *pair_
 	{
 	ctx->h_px.assign(pair_x, pair_x + npairs);
 	ctx->h_py.assign(pair_y, pair_y + npairs);
-	ctx->store_allpairs = false;
-	ctx->ea_allpairs = false;
-	ctx->store_valid = false;
-	ctx->plan_valid = false;
-	ctx->plan_is_allpairs = false;
+	mb_store_set_pairs(ctx, PAIRS_LIST);
 	}
 
 int mb200_posteriors(mb200_ctx *ctx, uint32_t npairs, const uint32_t *pair_x, const uint32_t *pair_y,
@@ -765,23 +752,14 @@ int mb200_posteriors_allpairs(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi, floa
 	if (p_lo >= p_hi || p_hi > npairs)
 		return mb_fail(ctx, MB200_EINVAL, "pair range [%u,%u) invalid for %llu pairs", p_lo, p_hi,
 		  (unsigned long long) npairs);
-	if (!(ctx->plan_valid && ctx->plan_is_allpairs && ctx->store_p_lo == p_lo && ctx->store_p_hi == p_hi))
+	const StoreState &s = ctx->store;
+	if (!(ctx->plan_valid && s.pairs == PAIRS_RANGE && s.p_lo == p_lo && s.p_hi == p_hi))
 		{
 		mb_allpairs_list(ctx->nseq, p_lo, p_hi, ctx->h_px, ctx->h_py);
-		ctx->plan_valid = false;
+		mb_store_set_pairs(ctx, PAIRS_RANGE, p_lo, p_hi);
 		}
-	ctx->store_valid = false;
-	ctx->ea_allpairs = false;
-	ctx->plan_is_allpairs = true;
-	ctx->store_p_lo = p_lo;
-	ctx->store_p_hi = p_hi;
-	const int rc = run_posteriors(ctx, ea_out, nullptr, 0);
-	if (rc == MB200_OK)
-		{
-		ctx->store_allpairs = (p_lo == 0 && p_hi == npairs);
-		ctx->ea_allpairs = ctx->store_allpairs;
-		}
-	return rc;
+	mb_store_drop(ctx);
+	return run_posteriors(ctx, ea_out, nullptr, 0);
 	}
 
 int mb200_calc_post_dense_pair(mb200_ctx *ctx, uint32_t npairs, const uint32_t *pair_x, const uint32_t *pair_y,
@@ -865,23 +843,7 @@ int mb200_store_npairs(const mb200_ctx *ctx, uint32_t *npairs)
 	{
 	if (!ctx || !npairs)
 		return MB200_EINVAL;
-	*npairs = ctx->store_valid ? (uint32_t) ctx->h_px.size() : 0;
-	return MB200_OK;
-	}
-
-static int fetch_store_index(mb200_ctx *ctx)
-	{
-	if (!ctx->store_valid)
-		return mb_fail(ctx, MB200_EINVAL, "no posterior store (run mb200_posteriors first)");
-	const size_t np = ctx->h_px.size();
-	if (ctx->h_nnz.size() == np && ctx->h_index_valid)
-		return MB200_OK;
-	ctx->h_nnz.resize(np);
-	ctx->h_entbase.resize(np);
-	CU(cudaMemcpyAsync(ctx->h_nnz.data(), ctx->d_nnz.p, np*sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
-	CU(cudaMemcpyAsync(ctx->h_entbase.data(), ctx->d_entbase.p, np*sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
-	CU(cudaStreamSynchronize(ctx->stream));
-	ctx->h_index_valid = true;
+	*npairs = ctx->store.present ? (uint32_t) ctx->h_px.size() : 0;
 	return MB200_OK;
 	}
 
@@ -890,8 +852,7 @@ int mb200_store_nnz(mb200_ctx *ctx, uint32_t *nnz_out, uint64_t *total_nnz)
 	if (!ctx)
 		return MB200_EINVAL;
 	cudaSetDevice(ctx->device);
-	ctx->h_index_valid = false;
-	const int rc = fetch_store_index(ctx);
+	const int rc = mb_store_require(ctx, "mb200_store_nnz", NEED_INDEX);
 	if (rc != MB200_OK)
 		return rc;
 	uint64_t tot = 0;
@@ -913,7 +874,7 @@ int mb200_export_pair(mb200_ctx *ctx, uint32_t pair, uint32_t *offsets, mb200_en
 	cudaSetDevice(ctx->device);
 	// the host index is re-read only when the store changed: at C3 it is 6 MB, and callers export
 	// pairs one at a time
-	int rc = fetch_store_index(ctx);
+	int rc = mb_store_require(ctx, "mb200_export_pair", NEED_INDEX);
 	if (rc != MB200_OK)
 		return rc;
 	if (pair >= ctx->h_px.size())

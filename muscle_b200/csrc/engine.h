@@ -13,6 +13,25 @@ struct DevBuf
 
 struct PostDebug { float *fwd, *bwd, *post, *total; uint32_t pair; };
 
+// What the sparse posterior store holds.  Only store.cu changes it (mb_store_* below).
+enum StorePairs { PAIRS_NONE, PAIRS_LIST, PAIRS_RANGE };     // h_px/h_py: none, a caller's list, all pairs [p_lo,p_hi)
+// derived forms in build order, each made from the one before: entries packed in store order without holes,
+// the transposed orientation, the column masks of both orientations (relax.cu)
+enum StoreForm { FORM_RAW, FORM_PACKED, FORM_TRANSPOSED, FORM_MASKED };
+struct StoreState
+	{
+	StorePairs pairs = PAIRS_NONE;
+	uint32_t p_lo = 0, p_hi = 0;
+	bool present = false;             // the device holds the store of that pair list
+	bool ea_here = false;             // d_ea holds the EA of all N(N-1)/2 pairs, computed on this device
+	StoreForm form = FORM_RAW;
+	bool index_valid = false;         // h_nnz / h_entbase match the device (always, once packed)
+	bool tr_stale = false;            // forward values changed since the transposed copy was refreshed
+	};
+// mb_store_require(needs): the StoreForm a consumer reads, or'ed with: the store holds all N(N-1)/2 pairs,
+// and their EA vector was computed here; the host index
+constexpr unsigned NEED_ALLPAIRS = 4, NEED_EA = 8, NEED_INDEX = 16;
+
 struct mb200_ctx
 	{
 	int device = 0;
@@ -40,14 +59,7 @@ struct mb200_ctx
 	DevBuf d_megaT, d_insP;
 
 	// the store: sparse posteriors of the listed pairs (replaces MPCFlat::m_SparsePosts1/2)
-	bool store_valid = false;
-	bool store_allpairs = false;      // holds all N(N-1)/2 pairs in reference order
-	bool ea_allpairs = false;         // d_ea holds the EA of all pairs (computed on this device)
-	uint32_t store_p_lo = 0, store_p_hi = 0;
-	bool store_packed = false;        // entries are packed in store order (entbase ascending, no holes)
-	bool store_tr_valid = false;      // transposed orientation + permutation built
-	bool tr_values_stale = false;     // forward values changed since the transposed copy was refreshed
-	bool store_masks_valid = false;   // column bit masks of both orientations built (relax.cu)
+	StoreState store;
 	std::vector<uint64_t> h_tr_rowbase;
 	uint64_t store_nnz = 0;
 	uint32_t nnz_per_row_cap = 12;    // entry pool sizing guess (retry with the exact count on overflow)
@@ -55,7 +67,6 @@ struct mb200_ctx
 	std::vector<uint64_t> h_rowbase;
 	std::vector<uint32_t> h_nnz;
 	std::vector<uint64_t> h_entbase;
-	bool h_index_valid = false;
 	DevBuf d_px, d_py, d_order, d_chain;    // d_order: pairs chain after chain; d_chain: offsets of the chains in it
 	DevBuf d_rowoff, d_rowbase, d_entries, d_cursor, d_entbase, d_nnz, d_ea;     // d_cursor: control block, see prepare_plan
 	DevBuf d_entries2;                // second value buffer for the Jacobi update
@@ -78,8 +89,8 @@ struct mb200_ctx
 	bool msa_valid = false;
 	uint32_t *h_pinned = nullptr;     // 64 words of pinned host memory for small read-backs
 
-	// cached launch plan of the posterior stage (depends only on the pair list)
-	bool plan_valid = false, plan_is_allpairs = false;
+	// cached launch plan of the posterior stage (depends only on the pair list; mb_store_set_pairs drops it)
+	bool plan_valid = false;
 	int plan_force_c = 0;
 	uint64_t plan_cells = 0, plan_est_entries = 0, last_used_entries = 0;
 	std::vector<std::vector<uint32_t>> plan_bins;                 // pairs per size class
@@ -104,9 +115,12 @@ int mb_fail(mb200_ctx *ctx, int code, const char *fmt, ...);
 	  "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
 #define ENSURE(buf, bytes) do { if ((buf).ensure(bytes) != 0) \
 	return mb_fail(ctx, MB200_ENOMEM, "device allocation of %zu bytes failed (%s)", (size_t)(bytes), #buf); } while (0)
-int mb_store_pack_inplace(mb200_ctx *ctx);
-int mb_store_build_transposed(mb200_ctx *ctx);
-int mb_store_refresh_transposed(mb200_ctx *ctx);
-int mb_store_build_masks(mb200_ctx *ctx);
+void mb_store_set_pairs(mb200_ctx *ctx, StorePairs pairs, uint32_t p_lo = 0, uint32_t p_hi = 0);
+void mb_store_drop(mb200_ctx *ctx);
+void mb_store_fresh(mb200_ctx *ctx, bool adopted);
+void mb_store_values_written(mb200_ctx *ctx);
+int mb_store_require(mb200_ctx *ctx, const char *who, unsigned needs);
+void mb_store_entry_range(const mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi, uint64_t *e_lo, uint64_t *e_hi);
+int mb_build_masks(mb200_ctx *ctx);             // relax.cu
 void mb_release_post_scratch(mb200_ctx *ctx);
 void mb_allpairs_list(uint32_t n, uint32_t p_lo, uint32_t p_hi, std::vector<uint32_t> &px, std::vector<uint32_t> &py);

@@ -389,8 +389,8 @@ int mb200_group_consistency_iter(mb200_group *g)
 		if (g->hi[r] == g->lo[r])
 			continue;
 		mb200_ctx *c = g->ctx[r];
-		const uint64_t e_lo = c->h_entbase[g->lo[r]];
-		const uint64_t e_hi = g->hi[r] < np ? c->h_entbase[g->hi[r]] : c->store_nnz;
+		uint64_t e_lo = 0, e_hi = 0;
+		mb_store_entry_range(c, g->lo[r], g->hi[r], &e_lo, &e_hi);
 		if (e_hi == e_lo)
 			continue;
 		bytes += (e_hi - e_lo)*sizeof(mb200_entry);

@@ -150,20 +150,11 @@ static int build_masks_one(mb200_ctx *ctx, uint32_t np, uint64_t nslots, const u
 	return MB200_OK;
 	}
 
-int mb_store_build_masks(mb200_ctx *ctx)
+// the column masks of both orientations of a transposed store (mb_store_require)
+int mb_build_masks(mb200_ctx *ctx)
 	{
-	if (!ctx->store_masks_valid)
-		{
-		CU(cudaStreamSynchronize(ctx->stream));
-		mb_release_post_scratch(ctx);
-		}
-	int rc = mb_store_build_transposed(ctx);
-	if (rc != MB200_OK)
-		return rc;
-	if (ctx->store_masks_valid)
-		return MB200_OK;
 	const uint32_t np = (uint32_t) ctx->h_px.size();
-	rc = build_masks_one(ctx, np, ctx->h_rowbase.back(), (const uint64_t *) ctx->d_rowbase.p, (const uint32_t *) ctx->d_rowoff.p,
+	int rc = build_masks_one(ctx, np, ctx->h_rowbase.back(), (const uint64_t *) ctx->d_rowbase.p, (const uint32_t *) ctx->d_rowoff.p,
 	  (const mb200_entry *) ctx->d_entries.p, ctx->d_mk_hdr, ctx->d_mk_words);
 	if (rc != MB200_OK)
 		return rc;
@@ -172,7 +163,6 @@ int mb_store_build_masks(mb200_ctx *ctx)
 	if (rc != MB200_OK)
 		return rc;
 	CU(cudaStreamSynchronize(ctx->stream));
-	ctx->store_masks_valid = true;
 	return MB200_OK;
 	}
 
@@ -202,12 +192,6 @@ struct ZDesc
 #ifndef RELAX_EPT
 #define RELAX_EPT 4          // entries per thread held in registers per sweep
 #endif
-
-__device__ __forceinline__ uint32_t pair_index(uint32_t n, uint32_t a, uint32_t b)
-	{
-	// row-major i<j (mpcflat.cpp:139-159): p = a*n - a(a+1)/2 + (b-a-1)
-	return (uint32_t)((uint64_t) a*n - (uint64_t) a*(a + 1)/2 + (b - a - 1));
-	}
 
 // MINB: resident CTAs/SM the register allocation is bounded for (sm_90a: 2: 96 registers, no spill;
 // 3: 80, no spill; 4: 64, 56 bytes spilled).  The kernel is bound by gather latency, so occupancy
@@ -282,23 +266,23 @@ k_relax(const RelaxParams P)
 					// S[x->z]: rows are positions of x
 					if (x < z)
 						{
-						const uint32_t q = pair_index(n, x, z);
+						const uint32_t q = mb_pair_index(n, x, z);
 						d.hdrA = P.hdr + P.rowbase[q]; d.wordsA = P.words; d.enA = P.entries + P.entbase[q];
 						}
 					else
 						{
-						const uint32_t q = pair_index(n, z, x);
+						const uint32_t q = mb_pair_index(n, z, x);
 						d.hdrA = P.trhdr + P.trbase[q]; d.wordsA = P.trwords; d.enA = P.trentries + P.entbase[q];
 						}
 					// S[y->z]: rows are positions of y
 					if (y < z)
 						{
-						const uint32_t q = pair_index(n, y, z);
+						const uint32_t q = mb_pair_index(n, y, z);
 						d.hdrB = P.hdr + P.rowbase[q]; d.wordsB = P.words; d.enB = P.entries + P.entbase[q];
 						}
 					else
 						{
-						const uint32_t q = pair_index(n, z, y);
+						const uint32_t q = mb_pair_index(n, z, y);
 						d.hdrB = P.trhdr + P.trbase[q]; d.wordsB = P.trwords; d.enB = P.trentries + P.entbase[q];
 						}
 					}
@@ -437,7 +421,7 @@ static int prepare_relax_order(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi)
 			for (uint32_t x = tx; x < std::min(n, tx + T); ++x)
 				for (uint32_t y = std::max(ty, x + 1); y < std::min(n, ty + T); ++y)
 					{
-					const uint32_t p = (uint32_t)((uint64_t) x*n - (uint64_t) x*(x + 1)/2 + (y - x - 1));
+					const uint32_t p = mb_pair_index(n, x, y);
 					if (p >= p_lo && p < p_hi)
 						order.push_back(p);
 					}
@@ -457,9 +441,9 @@ int mb200_consistency_iter(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi)
 	{
 	if (!ctx)
 		return MB200_EINVAL;
-	if (!ctx->store_valid || !ctx->store_allpairs)
-		return mb_fail(ctx, MB200_EINVAL, "mb200_consistency_iter: the store must hold all N(N-1)/2 pairs "
-		  "(mb200_posteriors_allpairs(0,npairs) or mb200_store_load_allpairs)");
+	int rc = mb_store_require(ctx, "mb200_consistency_iter", NEED_ALLPAIRS);
+	if (rc != MB200_OK)
+		return rc;
 	const uint32_t n = ctx->nseq;
 	const uint32_t np = (uint32_t) ctx->h_px.size();
 	if (p_lo > p_hi || p_hi > np)
@@ -469,16 +453,9 @@ int mb200_consistency_iter(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi)
 	cudaSetDevice(ctx->device);
 	cudaStream_t st = ctx->stream;
 	CU(cudaEventRecord(ctx->ev0, st));
-	int rc = mb_store_build_masks(ctx);        // packs, builds the transposed orientation and the masks once
+	rc = mb_store_require(ctx, "mb200_consistency_iter", NEED_ALLPAIRS | FORM_MASKED);
 	if (rc != MB200_OK)
 		return rc;
-	if (ctx->tr_values_stale)
-		{
-		rc = mb_store_refresh_transposed(ctx);
-		if (rc != MB200_OK)
-			return rc;
-		ctx->tr_values_stale = false;
-		}
 	ENSURE(ctx->d_entries2, (ctx->store_nnz + 64)*sizeof(mb200_entry));
 	CU(cudaEventRecord(ctx->ev1, st));
 	if (p_hi > p_lo)
@@ -517,8 +494,8 @@ int mb200_consistency_iter(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi)
 		}
 	CU(cudaEventRecord(ctx->ev2, st));
 	// pairs outside the range keep their old values until the peers' results arrive
-	const uint64_t e_lo = p_lo < np ? ctx->h_entbase[p_lo] : ctx->store_nnz;
-	const uint64_t e_hi = p_hi < np ? ctx->h_entbase[p_hi] : ctx->store_nnz;
+	uint64_t e_lo = 0, e_hi = 0;
+	mb_store_entry_range(ctx, p_lo, p_hi, &e_lo, &e_hi);
 	const int blocks = ctx->prop.multiProcessorCount*8;
 	if (e_lo > 0)
 		{
@@ -534,7 +511,7 @@ int mb200_consistency_iter(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi)
 	CU(cudaEventRecord(ctx->ev3, st));
 	CU(cudaStreamSynchronize(st));
 	std::swap(ctx->d_entries, ctx->d_entries2);            // consflat.cpp:22
-	ctx->tr_values_stale = true;
+	mb_store_values_written(ctx);
 	cudaEventElapsedTime(&ctx->stats.last_kernel_ms, ctx->ev1, ctx->ev2);
 	cudaEventElapsedTime(&ctx->stats.last_total_ms, ctx->ev0, ctx->ev3);
 	return MB200_OK;

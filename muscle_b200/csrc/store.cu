@@ -1,6 +1,6 @@
-// store.cu -- the device-resident sparse posterior store: packing in pair order (export and the
-// multi-GPU exchange image), loading a gathered image, values-only views, and the transposed
-// orientation that the consistency kernel needs.
+// store.cu -- the device-resident sparse posterior store: its state (StoreState, engine.h), packing in
+// pair order (export and the multi-GPU exchange image), loading a gathered image, values-only views,
+// and the transposed orientation that the consistency kernel and the joins need.
 //
 // Reference counterparts: the store replaces MPCFlat::m_SparsePosts1/2 (mpcflat.h:46-49); the wire
 // format of one pair is MySparseMx's (mysparsemx.h:6-98).  The transposed orientation replaces the
@@ -154,20 +154,80 @@ __global__ void k_refresh_transposed_pairs(uint32_t npairs, const uint64_t *__re
 	}
 
 // ---------------------------------------------------------------------------------------------
-// host helpers
-int mb_store_pack_inplace(mb200_ctx *ctx)
+// the store's state (StoreState, engine.h) and its derived forms
+static bool holds_allpairs(const mb200_ctx *ctx)
 	{
-	// make entbase the exclusive scan of nnz in store order (deterministic layout, no holes)
-	if (!ctx->store_valid)
-		return mb_fail(ctx, MB200_EINVAL, "no posterior store (run mb200_posteriors first)");
-	if (ctx->store_packed)
-		return MB200_OK;
+	const StoreState &s = ctx->store;
+	return s.pairs == PAIRS_RANGE && s.p_lo == 0 && s.p_hi == (uint64_t) ctx->nseq*(ctx->nseq - 1)/2;
+	}
+
+// h_px/h_py now hold another pair list (or none): the store and the posterior plan of the old one go
+void mb_store_set_pairs(mb200_ctx *ctx, StorePairs pairs, uint32_t p_lo, uint32_t p_hi)
+	{
+	ctx->store = StoreState{pairs, p_lo, p_hi};
+	ctx->plan_valid = false;
+	}
+
+// the inputs changed, or a posterior stage starts: the pair list and its plan stay
+void mb_store_drop(mb200_ctx *ctx)
+	{
+	ctx->store.present = false;
+	}
+
+// a new store of the current pair list: computed by the posterior stage (raw layout, with its EA
+// vector) or adopted as a packed image with its host index and no EA
+void mb_store_fresh(mb200_ctx *ctx, bool adopted)
+	{
+	StoreState &s = ctx->store;
+	s.present = true;
+	s.ea_here = !adopted && holds_allpairs(ctx);
+	s.form = adopted ? FORM_PACKED : FORM_RAW;
+	s.index_valid = adopted;
+	s.tr_stale = false;
+	}
+
+// the forward values changed in place (the pattern did not): the transposed copy is refreshed when next read
+void mb_store_values_written(mb200_ctx *ctx)
+	{
+	ctx->store.tr_stale = true;
+	}
+
+// entries [e_lo,e_hi) of the pairs [p_lo,p_hi) of a packed store
+void mb_store_entry_range(const mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi, uint64_t *e_lo, uint64_t *e_hi)
+	{
+	const size_t np = ctx->h_px.size();
+	*e_lo = p_lo < np ? ctx->h_entbase[p_lo] : ctx->store_nnz;
+	*e_hi = p_hi < np ? ctx->h_entbase[p_hi] : ctx->store_nnz;
+	}
+
+// h_nnz and, unless packing is about to compute them, h_entbase from the device
+static int read_index(mb200_ctx *ctx, bool entbase)
+	{
+	const size_t np = ctx->h_px.size();
+	ctx->h_nnz.resize(np);
+	CU(cudaMemcpyAsync(ctx->h_nnz.data(), ctx->d_nnz.p, np*sizeof(uint32_t), cudaMemcpyDeviceToHost, ctx->stream));
+	if (entbase)
+		{
+		ctx->h_entbase.resize(np);
+		CU(cudaMemcpyAsync(ctx->h_entbase.data(), ctx->d_entbase.p, np*sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
+		}
+	CU(cudaStreamSynchronize(ctx->stream));
+	ctx->store.index_valid = entbase;
+	return MB200_OK;
+	}
+
+// make entbase the exclusive scan of nnz in store order (deterministic layout, no holes)
+static int pack(mb200_ctx *ctx)
+	{
 	cudaSetDevice(ctx->device);
 	cudaStream_t st = ctx->stream;
 	const uint32_t np = (uint32_t) ctx->h_px.size();
-	ctx->h_nnz.resize(np);
-	CU(cudaMemcpyAsync(ctx->h_nnz.data(), ctx->d_nnz.p, np*sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-	CU(cudaStreamSynchronize(st));
+	if (!ctx->store.index_valid)
+		{
+		const int rc = read_index(ctx, false);
+		if (rc != MB200_OK)
+			return rc;
+		}
 	std::vector<uint64_t> base(np + 1, 0);
 	for (uint32_t k = 0; k < np; ++k)
 		base[k + 1] = base[k] + ctx->h_nnz[k];
@@ -184,21 +244,14 @@ int mb_store_pack_inplace(mb200_ctx *ctx)
 	CU(cudaStreamSynchronize(st));
 	std::swap(ctx->d_entries, ctx->d_entries2);
 	ctx->h_entbase.assign(base.begin(), base.begin() + np);
-	ctx->h_index_valid = true;
 	ctx->store_nnz = total;
-	ctx->store_packed = true;
-	ctx->store_tr_valid = false;
-	ctx->store_masks_valid = false;
+	ctx->store.index_valid = true;
+	ctx->store.form = FORM_PACKED;
 	return MB200_OK;
 	}
 
-int mb_store_build_transposed(mb200_ctx *ctx)
+static int build_transposed(mb200_ctx *ctx)
 	{
-	if (ctx->store_tr_valid)
-		return MB200_OK;
-	int rc = mb_store_pack_inplace(ctx);
-	if (rc != MB200_OK)
-		return rc;
 	cudaStream_t st = ctx->stream;
 	const uint32_t np = (uint32_t) ctx->h_px.size();
 	std::vector<uint64_t> trb(np + 1, 0);
@@ -219,11 +272,12 @@ int mb_store_build_transposed(mb200_ctx *ctx)
 	ctx->stats.kernel_launches++;
 	CU(cudaStreamSynchronize(st));
 	ctx->h_tr_rowbase = trb;
-	ctx->store_tr_valid = true;
+	ctx->store.form = FORM_TRANSPOSED;
+	ctx->store.tr_stale = false;
 	return MB200_OK;
 	}
 
-int mb_store_refresh_transposed(mb200_ctx *ctx)
+static int refresh_transposed(mb200_ctx *ctx)
 	{
 	const uint32_t np = (uint32_t) ctx->h_px.size();
 	const int blocks = ctx->prop.multiProcessorCount*8;
@@ -232,6 +286,44 @@ int mb_store_refresh_transposed(mb200_ctx *ctx)
 	  (mb200_entry *) ctx->d_tr_entries.p);
 	CU(cudaGetLastError());
 	ctx->stats.kernel_launches++;
+	ctx->store.tr_stale = false;
+	return MB200_OK;
+	}
+
+// Checks what `needs` asks of the store and builds the derived forms it lacks, in chain order
+int mb_store_require(mb200_ctx *ctx, const char *who, unsigned needs)
+	{
+	StoreState &s = ctx->store;
+	if ((needs & NEED_EA) && !(s.present && s.ea_here))
+		return mb_fail(ctx, MB200_EINVAL, "%s: no all-pairs EA vector on this device "
+		  "(mb200_posteriors_allpairs(0, npairs) must have run here, or pass ea)", who);
+	if ((needs & NEED_ALLPAIRS) && !(s.present && holds_allpairs(ctx)))
+		return mb_fail(ctx, MB200_EINVAL, "%s: the store must hold all N(N-1)/2 pairs "
+		  "(mb200_posteriors_allpairs(0,npairs) or mb200_store_load_allpairs)", who);
+	if (!s.present)
+		return mb_fail(ctx, MB200_EINVAL, "no posterior store (run mb200_posteriors first)");
+	const unsigned want = needs & 3;
+	int rc = MB200_OK;
+	if (want == FORM_MASKED && s.form < FORM_MASKED)
+		{
+		// the posterior scratch goes first: at C3 both stages fit one 80 GB device only without it
+		CU(cudaStreamSynchronize(ctx->stream));
+		mb_release_post_scratch(ctx);
+		}
+	if (want >= FORM_PACKED && s.form < FORM_PACKED && (rc = pack(ctx)) != MB200_OK)
+		return rc;
+	if (want >= FORM_TRANSPOSED && s.form < FORM_TRANSPOSED && (rc = build_transposed(ctx)) != MB200_OK)
+		return rc;
+	if (want >= FORM_TRANSPOSED && s.tr_stale && (rc = refresh_transposed(ctx)) != MB200_OK)
+		return rc;
+	if (want == FORM_MASKED && s.form < FORM_MASKED)
+		{
+		if ((rc = mb_build_masks(ctx)) != MB200_OK)
+			return rc;
+		s.form = FORM_MASKED;
+		}
+	if ((needs & NEED_INDEX) && !s.index_valid && (rc = read_index(ctx, true)) != MB200_OK)
+		return rc;
 	return MB200_OK;
 	}
 
@@ -242,7 +334,7 @@ int mb200_store_pack(mb200_ctx *ctx, const uint32_t **d_offsets, uint64_t *n_off
 	{
 	if (!ctx)
 		return MB200_EINVAL;
-	const int rc = mb_store_pack_inplace(ctx);
+	const int rc = mb_store_require(ctx, "mb200_store_pack", FORM_PACKED);
 	if (rc != MB200_OK)
 		return rc;
 	if (d_offsets)
@@ -260,7 +352,7 @@ int mb200_export_all(mb200_ctx *ctx, uint32_t *offsets_concat, mb200_entry *entr
 	{
 	if (!ctx || !offsets_concat || !entries_concat)
 		return mb_fail(ctx, MB200_EINVAL, "mb200_export_all: NULL argument");
-	const int rc = mb_store_pack_inplace(ctx);
+	const int rc = mb_store_require(ctx, "mb200_export_all", FORM_PACKED);
 	if (rc != MB200_OK)
 		return rc;
 	CU(cudaMemcpy(offsets_concat, ctx->d_rowoff.p, ctx->h_rowbase.back()*sizeof(uint32_t), cudaMemcpyDeviceToHost));
@@ -297,7 +389,6 @@ int mb200_store_exchange_begin(mb200_ctx *ctx, uint64_t n_offsets, uint64_t n_en
 static int adopt_image(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi, uint64_t n_offsets, uint64_t n_entries)
 	{
 	cudaStream_t st = ctx->stream;
-	const uint64_t all = (uint64_t) ctx->nseq*(ctx->nseq - 1)/2;
 	std::vector<uint32_t> px, py;
 	mb_allpairs_list(ctx->nseq, p_lo, p_hi, px, py);
 	const uint32_t np = (uint32_t) px.size();
@@ -345,19 +436,9 @@ static int adopt_image(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi, uint64_t n_
 	ctx->h_rowbase.swap(rowbase);
 	ctx->h_nnz.swap(h_nnz);
 	ctx->h_entbase.swap(h_entbase);
-	ctx->plan_valid = false;
-	ctx->h_index_valid = true;
 	ctx->store_nnz = tot;
-	ctx->store_valid = true;
-	ctx->store_packed = true;
-	ctx->store_tr_valid = false;
-	ctx->store_masks_valid = false;
-	ctx->tr_values_stale = false;
-	ctx->store_allpairs = (p_lo == 0 && p_hi == all);
-	ctx->ea_allpairs = false;          // the adopted image carries no EA values
-	ctx->plan_is_allpairs = false;
-	ctx->store_p_lo = p_lo;
-	ctx->store_p_hi = p_hi;
+	mb_store_set_pairs(ctx, PAIRS_RANGE, p_lo, p_hi);
+	mb_store_fresh(ctx, true);
 	return MB200_OK;
 	}
 
@@ -396,7 +477,7 @@ int mb200_store_entries_ptr(mb200_ctx *ctx, mb200_entry **d_entries, uint64_t *n
 	{
 	if (!ctx || !d_entries)
 		return mb_fail(ctx, MB200_EINVAL, "mb200_store_entries_ptr: NULL argument");
-	const int rc = mb_store_pack_inplace(ctx);
+	const int rc = mb_store_require(ctx, "mb200_store_entries_ptr", FORM_PACKED);
 	if (rc != MB200_OK)
 		return rc;
 	*d_entries = (mb200_entry *) ctx->d_entries.p;
@@ -407,9 +488,9 @@ int mb200_store_entries_ptr(mb200_ctx *ctx, mb200_entry **d_entries, uint64_t *n
 
 int mb200_store_values_changed(mb200_ctx *ctx)
 	{
-	if (!ctx || !ctx->store_valid)
+	if (!ctx || !ctx->store.present)
 		return mb_fail(ctx, MB200_EINVAL, "mb200_store_values_changed: no store");
-	ctx->tr_values_stale = true;
+	mb_store_values_written(ctx);
 	return MB200_OK;
 	}
 
@@ -417,7 +498,7 @@ int mb200_store_values(mb200_ctx *ctx, float *d_values_out, uint64_t n_entries)
 	{
 	if (!ctx || !d_values_out)
 		return mb_fail(ctx, MB200_EINVAL, "mb200_store_values: NULL argument");
-	const int rc = mb_store_pack_inplace(ctx);
+	const int rc = mb_store_require(ctx, "mb200_store_values", FORM_PACKED);
 	if (rc != MB200_OK)
 		return rc;
 	if (n_entries != ctx->store_nnz)
@@ -435,7 +516,8 @@ int mb200_store_set_values(mb200_ctx *ctx, const float *d_values, uint64_t first
 	{
 	if (!ctx || !d_values)
 		return mb_fail(ctx, MB200_EINVAL, "mb200_store_set_values: NULL argument");
-	if (!ctx->store_valid || !ctx->store_packed)
+	// refused rather than packed here: first_entry refers to the packed layout
+	if (!ctx->store.present || ctx->store.form < FORM_PACKED)
 		return mb_fail(ctx, MB200_EINVAL, "mb200_store_set_values: store must be packed (mb200_store_pack)");
 	if (first_entry + n_entries > ctx->store_nnz)
 		return mb_fail(ctx, MB200_EINVAL, "value range out of bounds");
@@ -444,7 +526,7 @@ int mb200_store_set_values(mb200_ctx *ctx, const float *d_values, uint64_t first
 	CU(cudaGetLastError());
 	ctx->stats.kernel_launches++;
 	CU(cudaStreamSynchronize(ctx->stream));
-	ctx->tr_values_stale = true;
+	mb_store_values_written(ctx);
 	return MB200_OK;
 	}
 

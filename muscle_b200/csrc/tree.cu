@@ -212,9 +212,9 @@ extern "C" int mb200_guide_tree(mb200_ctx *ctx, const float *ea, int linkage, ui
 	else
 		{
 		// the EA vector the posterior stage left on this device (store order == all-pairs order)
-		if (!ctx->store_valid || !ctx->ea_allpairs)
-			return mb_fail(ctx, MB200_EINVAL, "mb200_guide_tree: no all-pairs EA vector on this device "
-			  "(mb200_posteriors_allpairs(0, npairs) must have run here, or pass ea)");
+		const int rc = mb_store_require(ctx, "mb200_guide_tree", NEED_EA);
+		if (rc != MB200_OK)
+			return rc;
 		d_ea = (const float *) ctx->d_ea.p;
 		}
 	P.ea = d_ea;

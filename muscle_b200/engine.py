@@ -76,8 +76,51 @@ def _ptr(a):
 	return C.c_void_p(a.ctypes.data) if a is not None else None
 
 
-class Engine:
+class _Inputs:
+	"""set_hmm, set_seqs and set_seqs_mega of an Engine or a Group: the same arguments go to mb200_<name> or
+	mb200_group_<name> (`_api`) of the context or group `_handle`"""
+	_api = None
+
+	def _set(self, name, *args):
+		self._ck(getattr(self.lib, self._api + name)(self._handle, *args))
+
+	def set_hmm(self, tables):
+		s = np.ascontiguousarray(tables["start"], np.float32)
+		t = np.ascontiguousarray(tables["trans"], np.float32).reshape(-1)
+		i = np.ascontiguousarray(tables["ins"], np.float32)
+		m = np.ascontiguousarray(tables["match"], np.float32).reshape(-1)
+		assert s.size == 5 and t.size == 25 and i.size == 256 and m.size == 65536
+		self._set("set_hmm", _ptr(s), _ptr(t), _ptr(i), _ptr(m), C.c_float(float(np.float32(tables["min_sparse_score"]))))
+
+	def set_seqs(self, seqs):
+		bs = [s if isinstance(s, (bytes, bytearray)) else s.encode() for s in seqs]
+		self.lens = np.array([len(b) for b in bs], np.int64)
+		off = np.zeros(len(bs) + 1, np.uint64)
+		off[1:] = np.cumsum(self.lens)
+		buf = np.frombuffer(b"".join(bs), dtype=np.uint8)
+		self.nseq = len(bs)
+		self._set("set_seqs", C.c_uint32(len(bs)), _ptr(buf), _ptr(off))
+
+	def set_seqs_mega(self, model, profiles):
+		"""Mega feature profiles: model = dict(alpha[F], weights[F], logprobs, logprobmx), profiles = list of
+		uint8 arrays [L][F] (Mega::m_Profiles)"""
+		F = len(model["alpha"])
+		alpha = np.ascontiguousarray(model["alpha"], np.uint32)
+		w = np.ascontiguousarray(model["weights"], np.float32)
+		lp = np.ascontiguousarray(model["logprobs"], np.float32)
+		lpm = np.ascontiguousarray(model["logprobmx"], np.float32)
+		self.lens = np.array([len(p) for p in profiles], np.int64)
+		off = np.zeros(len(profiles) + 1, np.uint64)
+		off[1:] = np.cumsum(self.lens)
+		let = np.ascontiguousarray(np.concatenate([np.asarray(p, np.uint8).reshape(-1, F) for p in profiles]), np.uint8)
+		self.nseq = len(profiles)
+		self._set("set_seqs_mega", C.c_uint32(self.nseq), _ptr(let), _ptr(off), C.c_uint32(F), _ptr(alpha), _ptr(w),
+		  _ptr(lp), _ptr(lpm))
+
+
+class Engine(_Inputs):
 	"""One context on one CUDA device (mb200_create .. mb200_destroy)."""
+	_api = "mb200_"
 
 	def __init__(self, device=0, _borrowed=None):
 		self.lib = load_library()
@@ -105,44 +148,13 @@ class Engine:
 		except Exception:
 			pass
 
+	@property
+	def _handle(self):
+		return self.h
+
 	def _ck(self, rc):
 		if rc != 0:
 			raise MB200Error(rc, self.lib.mb200_last_error(self.h).decode())
-
-	# ---- inputs
-	def set_hmm(self, tables):
-		s = np.ascontiguousarray(tables["start"], np.float32)
-		t = np.ascontiguousarray(tables["trans"], np.float32).reshape(-1)
-		i = np.ascontiguousarray(tables["ins"], np.float32)
-		m = np.ascontiguousarray(tables["match"], np.float32).reshape(-1)
-		assert s.size == 5 and t.size == 25 and i.size == 256 and m.size == 65536
-		self._ck(self.lib.mb200_set_hmm(self.h, _ptr(s), _ptr(t), _ptr(i), _ptr(m),
-		  C.c_float(float(np.float32(tables["min_sparse_score"])))))
-
-	def set_seqs(self, seqs):
-		bs = [s if isinstance(s, (bytes, bytearray)) else s.encode() for s in seqs]
-		self.lens = np.array([len(b) for b in bs], np.int64)
-		off = np.zeros(len(bs) + 1, np.uint64)
-		off[1:] = np.cumsum(self.lens)
-		buf = np.frombuffer(b"".join(bs), dtype=np.uint8)
-		self.nseq = len(bs)
-		self._ck(self.lib.mb200_set_seqs(self.h, C.c_uint32(len(bs)), _ptr(buf), _ptr(off)))
-
-	def set_seqs_mega(self, model, profiles):
-		"""Mega feature profiles: model = dict(alpha[F], weights[F], logprobs, logprobmx), profiles = list of
-		uint8 arrays [L][F] (Mega::m_Profiles)"""
-		F = len(model["alpha"])
-		alpha = np.ascontiguousarray(model["alpha"], np.uint32)
-		w = np.ascontiguousarray(model["weights"], np.float32)
-		lp = np.ascontiguousarray(model["logprobs"], np.float32)
-		lpm = np.ascontiguousarray(model["logprobmx"], np.float32)
-		self.lens = np.array([len(p) for p in profiles], np.int64)
-		off = np.zeros(len(profiles) + 1, np.uint64)
-		off[1:] = np.cumsum(self.lens)
-		let = np.ascontiguousarray(np.concatenate([np.asarray(p, np.uint8).reshape(-1, F) for p in profiles]), np.uint8)
-		self.nseq = len(profiles)
-		self._ck(self.lib.mb200_set_seqs_mega(self.h, C.c_uint32(self.nseq), _ptr(let), _ptr(off), C.c_uint32(F), _ptr(alpha),
-		  _ptr(w), _ptr(lp), _ptr(lpm)))
 
 	# ---- posterior stage
 	def posteriors(self, pair_x, pair_y, want_ea=True, force_c=0):
@@ -364,8 +376,9 @@ class Engine:
 		return {f: getattr(s, f) for f, _ in Stats._fields_}
 
 
-class Group:
+class Group(_Inputs):
 	"""Several GPUs driven by one process (mb200_group_*): what `muscle_b200 -align` uses."""
+	_api = "mb200_group_"
 
 	def __init__(self, devices=None):
 		self.lib = load_library()
@@ -393,6 +406,10 @@ class Group:
 		except Exception:
 			pass
 
+	@property
+	def _handle(self):
+		return self.g
+
 	def _ck(self, rc):
 		if rc != 0:
 			raise MB200Error(rc, self.lib.mb200_group_last_error(self.g).decode())
@@ -405,38 +422,6 @@ class Group:
 		px, py = np.triu_indices(n, 1)
 		e._pairs = (px.astype(np.uint32), py.astype(np.uint32))
 		return e
-
-	def set_hmm(self, tables):
-		s = np.ascontiguousarray(tables["start"], np.float32)
-		t = np.ascontiguousarray(tables["trans"], np.float32).reshape(-1)
-		i = np.ascontiguousarray(tables["ins"], np.float32)
-		m = np.ascontiguousarray(tables["match"], np.float32).reshape(-1)
-		self._ck(self.lib.mb200_group_set_hmm(self.g, _ptr(s), _ptr(t), _ptr(i), _ptr(m),
-		  C.c_float(float(np.float32(tables["min_sparse_score"])))))
-
-	def set_seqs(self, seqs):
-		bs = [s if isinstance(s, (bytes, bytearray)) else s.encode() for s in seqs]
-		self.lens = np.array([len(b) for b in bs], np.int64)
-		off = np.zeros(len(bs) + 1, np.uint64)
-		off[1:] = np.cumsum(self.lens)
-		buf = np.frombuffer(b"".join(bs), dtype=np.uint8)
-		self.nseq = len(bs)
-		self._ck(self.lib.mb200_group_set_seqs(self.g, C.c_uint32(len(bs)), _ptr(buf), _ptr(off)))
-
-	def set_seqs_mega(self, model, profiles):
-		"""Mega feature profiles on every member: the arguments of Engine.set_seqs_mega"""
-		F = len(model["alpha"])
-		alpha = np.ascontiguousarray(model["alpha"], np.uint32)
-		w = np.ascontiguousarray(model["weights"], np.float32)
-		lp = np.ascontiguousarray(model["logprobs"], np.float32)
-		lpm = np.ascontiguousarray(model["logprobmx"], np.float32)
-		self.lens = np.array([len(p) for p in profiles], np.int64)
-		off = np.zeros(len(profiles) + 1, np.uint64)
-		off[1:] = np.cumsum(self.lens)
-		let = np.ascontiguousarray(np.concatenate([np.asarray(p, np.uint8).reshape(-1, F) for p in profiles]), np.uint8)
-		self.nseq = len(profiles)
-		self._ck(self.lib.mb200_group_set_seqs_mega(self.g, C.c_uint32(self.nseq), _ptr(let), _ptr(off), C.c_uint32(F),
-		  _ptr(alpha), _ptr(w), _ptr(lp), _ptr(lpm)))
 
 	def posteriors_allpairs(self, want_ea=True):
 		n = self.nseq
