@@ -18,6 +18,15 @@
 #define MB_SM_ARRAYS_MEGA 7             // MEGA: float4 state + {letters 0..3, eY} + letters 4..7
 #define MB_CHAIN_MAX 32                 // posterior kernel: pairs in one chain (one per lane when the chain is read)
 #define MB_CHAIN_BUF (MB_CHAIN_MAX*38)  // words of per-warp chain scratch: kept counts [pair][lane], totals [pair], final cells [pair][5]
+#define MB_PLAIN_ROWS 2                 // posterior kernel: rows per lane per step of the plain-mode passes (MEGA: 1)
+
+// Forward steps one lane spends on a pair of LX rows at R rows per step: rows 0..LX, then one separator
+// step.  At R = 2 a pair of even LX starts with one all-LOG_ZERO row (-1), so that its rows pair up as
+// (LX-1, LX), (LX-3, LX-2), ... in Forward and Backward alike.
+__host__ __device__ __forceinline__ uint32_t mb_fwd_steps(uint32_t LX, int R)
+	{
+	return R == 1 ? LX + 2 : LX/2 + 2;
+	}
 
 // index of pair (a,b), a < b, in the row-major all-pairs order of the store (mpcflat.cpp:139-159)
 __host__ __device__ __forceinline__ uint32_t mb_pair_index(uint32_t n, uint32_t a, uint32_t b)
@@ -181,7 +190,7 @@ struct PostParams
 	uint8_t     *rowcnt;  size_t rowcnt_stride;  // bytes
 	uint32_t    *chainbuf;                       // MB_CHAIN_BUF words per warp
 	uint32_t     lxmax;                          // rows of one pair the scratch was sized for
-	uint32_t     fm_rows;                        // (lxmax+33): steps per strip slot in fm
+	uint32_t     fm_rows;                        // mb_fwd_steps(lxmax, R) + 31: steps per strip slot in fm (R*W floats each)
 	uint32_t     cmax;                           // k_posterior_sm: cap on the columns per lane (<= the size class)
 	// outputs
 	uint32_t       *rowoff;         // concatenated, pair k at rowbase[k], LX+1 entries

@@ -456,12 +456,13 @@ static int prepare_plan(mb200_ctx *ctx, int force_c)
 	ctx->plan_lxmax.assign(MB_MAX_C + 1, 0);
 	ctx->plan_lymax.assign(MB_MAX_C + 1, 0);
 	ctx->plan_fmax.assign(MB_MAX_C + 1, 0);
+	ctx->plan_fsteps.assign(MB_MAX_C + 1, 0);
 	ctx->plan_rmax.assign(MB_MAX_C + 1, 0);
 	std::vector<int> open(ctx->nseq, -1);
 	for (int C = 1; C <= MB_MAX_C; ++C)
 		{
 		std::vector<std::vector<uint32_t>> chains;
-		std::vector<uint64_t> frows, cost;
+		std::vector<uint64_t> frows, fsteps, cost;
 		for (uint32_t k : bins[C])
 			{
 			const uint32_t x = ctx->h_px[k], y = ctx->h_py[k];
@@ -472,14 +473,17 @@ static int prepare_plan(mb200_ctx *ctx, int force_c)
 				c = (int) chains.size();
 				chains.emplace_back();
 				frows.push_back(0);
+				fsteps.push_back(0);
 				cost.push_back(0);
 				}
 			chains[c].push_back(k);
 			frows[c] += LX + 2;
+			fsteps[c] += mb_fwd_steps(LX, MB_PLAIN_ROWS);
 			cost[c] += (uint64_t) LX*LY;
 			ctx->plan_lxmax[C] = std::max(ctx->plan_lxmax[C], LX);
 			ctx->plan_lymax[C] = std::max(ctx->plan_lymax[C], LY);
 			ctx->plan_fmax[C] = std::max<uint64_t>(ctx->plan_fmax[C], frows[c]);
+			ctx->plan_fsteps[C] = std::max<uint64_t>(ctx->plan_fsteps[C], fsteps[c]);
 			ctx->plan_rmax[C] = std::max<uint64_t>(ctx->plan_rmax[C], frows[c] - 2*chains[c].size());
 			}
 		for (uint32_t k : bins[C])
@@ -586,10 +590,12 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 			PostParams P;
 			memset(&P, 0, sizeof P);
 			P.lxmax = lxmax;
-			// Forward-M spill: a strip slot of fm_rows steps per strip of a single pair, or the steps of
-			// a chain (at most its Forward rows + 30), which always has one strip
-			P.fm_rows = lxmax + 33;
-			P.fm_stride = std::max<size_t>((size_t) nstrips*P.fm_rows, ctx->plan_fmax[C] + 31)*W;
+			// Forward-M spill, R rows of W columns per step: a strip slot of fm_rows steps per strip of a
+			// single pair, or the steps of a chain (at most its Forward steps + 30), which always has one strip
+			const int R = mega ? 1 : MB_PLAIN_ROWS;
+			P.fm_rows = mb_fwd_steps(lxmax, R) + 31;
+			P.fm_stride = std::max<size_t>((size_t) nstrips*P.fm_rows,
+			  (R == 1 ? ctx->plan_fmax[C] : ctx->plan_fsteps[C]) + 31)*R*W;
 			P.edge_stride = 2*((size_t) lxmax + 2);
 			P.rows_stride = (size_t) ctx->plan_rmax[C]*MB_CAP;
 			P.rowcnt_stride = ((size_t) ctx->plan_rmax[C] + 31)/16*16;

@@ -96,6 +96,7 @@ struct mb200_ctx
 	std::vector<std::vector<uint32_t>> plan_bins;                 // pairs per size class
 	std::vector<uint32_t> plan_bin_start, plan_lxmax, plan_lymax;  // bin_start: first chain of each size class
 	std::vector<uint64_t> plan_fmax, plan_rmax;                    // largest chain: Forward rows (sum of LX+2), rows (sum of LX)
+	std::vector<uint64_t> plan_fsteps;                             // largest chain: Forward steps at MB_PLAIN_ROWS rows per step
 
 	// per-warp scratch of the posterior kernel, one buffer per bin (PostParams fm, edge, rows, rowcnt, chainbuf)
 	DevBuf d_post_scratch[MB_MAX_C + 1];

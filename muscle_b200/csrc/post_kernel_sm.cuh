@@ -52,11 +52,10 @@
 #pragma once
 #include "common.cuh"
 
-// resident CTAs/SM the register budget is tuned for (64K registers: <= 85 per thread at 6, <= 102 at 5).
-// At 5 words per (column, lane) six CTAs of the classes up to 12 fit in an SM's shared memory; 14 and 16
-// do not, so they keep the budget of 5.
-#define MB_SM_BLOCKS 6
-#define MB_SM_BLOCKS_WIDE 5
+// resident CTAs/SM the plain-mode register budget is tuned for (64K registers: <= 102 per thread at 5,
+// 128 at 4).  The row-pair passes need about 96 registers; at 5 words per (column, lane) five CTAs of the
+// classes up to 14 fit in an SM's shared memory, and four of class 16, which therefore gets 128.
+#define MB_SM_BLOCKS 5
 
 // sum over features of the pre-multiplied pair tables, in feature order starting from 0
 // (mega.cpp:350-357); xb[f] = offset of row a_f of feature f's table, y0/y1 = packed letters of the column
@@ -142,6 +141,9 @@ __device__ __forceinline__ float2 mb_col_emit(const float *matchT, const MbXEmit
 		}
 	return xe.merow[*y2p];
 	}
+
+// the five values of a Backward cell (bwdflat3.cpp:95-125)
+struct MbBwdCell { float m, ix, jx, iy, jy; };
 
 // one strip of a chain: j0, the position in Y of its first column; nl, the lanes that hold columns of it;
 // cn, the lane's columns up to LY
@@ -485,10 +487,12 @@ __device__ void mb_compact_ea(const PostParams &P, uint32_t pair, int LX, int LY
 
 // CM: size class (columns per lane the shared memory is sized for; P.cmax <= CM caps C at run time)
 template <bool MEGA, int CM, bool DUMP>
-__global__ void __launch_bounds__(32*MB_WARPS_PER_BLOCK, MEGA ? 4 : (CM <= 12 ? MB_SM_BLOCKS : MB_SM_BLOCKS_WIDE))
+__global__ void __launch_bounds__(32*MB_WARPS_PER_BLOCK, (MEGA || CM > 14) ? 4 : MB_SM_BLOCKS)
 k_posterior_sm(const PostParams P)
 	{
 	constexpr int NARR = MEGA ? MB_SM_ARRAYS_MEGA : MB_SM_ARRAYS;
+	constexpr int R = MEGA ? 1 : MB_PLAIN_ROWS;       // rows per lane per step of Forward and Backward
+	static_assert(R == 1 || R == 2, "the passes are written for one row or a pair of rows per step");
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	PostSmemHdr &sm = *reinterpret_cast<PostSmemHdr *>(smem_raw);
 	const MbHmm h = P.h;
@@ -548,6 +552,7 @@ k_posterior_sm(const PostParams P)
 		const MbSeq Y = mb_seq(P, P.py[cpairs[0]]);
 		const int LY = Y.len;
 		const int sumLX = __reduce_add_sync(MB_FULL, lane < nch ? P.seqlen[P.px[cpairs[lane]]] : 0u);
+		const int sumFS = R == 1 ? 0 : __reduce_add_sync(MB_FULL, lane < nch ? mb_fwd_steps(P.seqlen[P.px[cpairs[lane]]], R) : 0u);
 		const int C = min(min(CM, (int) P.cmax), (LY + 31) >> 5);   // columns per lane for this chain
 		const MbStrips g = mb_strips(LY, C);               // more than one strip only for a chain of one pair
 		const int W = g.W;
@@ -560,117 +565,273 @@ k_posterior_sm(const PostParams P)
 		// separator step that resets the lane's state records to LOG_ZERO and passes LOG_ZERO on, so
 		// that row 0 of the next pair sees exactly the border of a fresh pair.  Pair k starts at chain
 		// step Fk + l, Fk = sum over earlier pairs of (LX + 2).
-		for (int strip = 0; strip < g.n; ++strip)
-			{
-			const auto [j0, nl, cn, last] = g.at(strip, lane);
-			const auto [edgeIn, edgeOut] = mb_strip_edges(edge0, edge1, strip);
-			float *fms = fm + (size_t) strip*P.fm_rows*W;
-
-			mb_stage_y<MEGA>(Y, j0 + lane*C, C, lane, h.pad, st, ye, y2);
-			float outM = Z, outAIY = Z, outAJY = Z, outS = Z;
-			float dprev = Z;
-			float bIX = Z, bJX = Z;
-			const int nsteps = sumLX + 2*nch - 2 + nl;
-			int kp = 0, r0 = lane;                // the lane's pair and the step of its row 0
-			MbSeq X = mb_seq(P, P.px[cpairs[0]]);
-			MbXRow xPref = mb_x_row<MEGA>(X, false, 0, h.pad);
-			for (int t = 0; t < nsteps; ++t)
+		if constexpr (R == 1)
+			for (int strip = 0; strip < g.n; ++strip)
 				{
-				const int i = t - r0;
-				const MbXRow x = xPref;
-				xPref = mb_x_row<MEGA>(X, i >= 0 && i < X.len, i, h.pad);
-				float Lm = __shfl_up_sync(MB_FULL, outM, 1);
-				float Laiy = __shfl_up_sync(MB_FULL, outAIY, 1);
-				float Lajy = __shfl_up_sync(MB_FULL, outAJY, 1);
-				float Ls = __shfl_up_sync(MB_FULL, outS, 1);
-				if (i >= 0 && i <= X.len && lane < nl)
+				const auto [j0, nl, cn, last] = g.at(strip, lane);
+				const auto [edgeIn, edgeOut] = mb_strip_edges(edge0, edge1, strip);
+				float *fms = fm + (size_t) strip*P.fm_rows*W;
+
+				mb_stage_y<MEGA>(Y, j0 + lane*C, C, lane, h.pad, st, ye, y2);
+				float outM = Z, outAIY = Z, outAJY = Z, outS = Z;
+				float dprev = Z;
+				float bIX = Z, bJX = Z;
+				const int nsteps = sumLX + 2*nch - 2 + nl;
+				int kp = 0, r0 = lane;                // the lane's pair and the step of its row 0
+				MbSeq X = mb_seq(P, P.px[cpairs[0]]);
+				MbXRow xPref = mb_x_row<MEGA>(X, false, 0, h.pad);
+				for (int t = 0; t < nsteps; ++t)
 					{
-					const MbXEmit xe = mb_x_emit<MEGA>(P, sm.insT, meT, h.KS, x);
-					const float ex = xe.ins;
-					if (lane == 0)
+					const int i = t - r0;
+					const MbXRow x = xPref;
+					xPref = mb_x_row<MEGA>(X, i >= 0 && i < X.len, i, h.pad);
+					float Lm = __shfl_up_sync(MB_FULL, outM, 1);
+					float Laiy = __shfl_up_sync(MB_FULL, outAIY, 1);
+					float Lajy = __shfl_up_sync(MB_FULL, outAJY, 1);
+					float Ls = __shfl_up_sync(MB_FULL, outS, 1);
+					if (i >= 0 && i <= X.len && lane < nl)
 						{
-						if (strip == 0)
+						const MbXEmit xe = mb_x_emit<MEGA>(P, sm.insT, meT, h.KS, x);
+						const float ex = xe.ins;
+						if (lane == 0)
 							{
-							Lm = Z;
-							if (i == 0)
+							if (strip == 0)
 								{
-								Laiy = h.tSI; Lajy = h.tSJ; Ls = h.tSM;
-								}
-							else
-								{
-								if (i == 1)
+								Lm = Z;
+								if (i == 0)
 									{
-									bIX = ADD(h.tSI, ex); bJX = ADD(h.tSJ, ex);
+									Laiy = h.tSI; Lajy = h.tSJ; Ls = h.tSM;
 									}
 								else
 									{
-									bIX = ADD(ADD(bIX, h.tII), ex); bJX = ADD(ADD(bJX, h.tJJ), ex);
+									if (i == 1)
+										{
+										bIX = ADD(h.tSI, ex); bJX = ADD(h.tSJ, ex);
+										}
+									else
+										{
+										bIX = ADD(ADD(bIX, h.tII), ex); bJX = ADD(ADD(bJX, h.tJJ), ex);
+										}
+									Laiy = Z; Lajy = Z;
+									Ls = la(ADD(bIX, h.tIM), ADD(bJX, h.tJM));
 									}
-								Laiy = Z; Lajy = Z;
-								Ls = la(ADD(bIX, h.tIM), ADD(bJX, h.tJM));
 								}
+							else
+								{
+								const float4 e = edgeIn[i];
+								Lm = e.x; Laiy = e.y; Lajy = e.z; Ls = e.w;
+								}
+							}
+						float diag = dprev;
+						dprev = Ls;
+						float lm = Lm, laiy = Laiy, lajy = Lajy, sLast = Z;
+						float ix = Z, jx = Z, iy = Z, jy = Z;
+						float4 *sp = st + lane;
+						const uint2 *yp = ye + lane;
+						const uint32_t *y2p = y2 + lane;
+						float *dst = fms + (size_t) t*W + lane;
+						const bool dump = DUMP && i >= 1 && cpairs[kp] == P.dbg_pair;
+#pragma unroll 1
+						for (int c = 0; c < cn; ++c, sp += 32, yp += 32, y2p += 32, dst += 32)
+							{
+							const float4 v = *sp;                      // {S, M, IX, JX} of row i-1
+							const auto [em, eyc] = mb_col_emit<MEGA>(matchT, xe, nf, yp, y2p);
+							const float m = ADD(diag, em);
+							ix = ADD(la(ADD(v.z, h.tII), ADD(v.y, h.tMI)), ex);
+							jx = ADD(la(ADD(v.w, h.tJJ), ADD(v.y, h.tMJ)), ex);
+							iy = ADD(la(laiy, ADD(lm, h.tMI)), eyc);
+							jy = ADD(la(lajy, ADD(lm, h.tMJ)), eyc);
+							const float s = la(ADD(m, h.tMM), la(ADD(ix, h.tIM), la(ADD(jx, h.tJM),
+							  la(ADD(iy, h.tIM), ADD(jy, h.tJM)))));
+							diag = v.x;
+							*sp = make_float4(s, m, ix, jx);
+							lm = m;
+							laiy = ADD(iy, h.tII);
+							lajy = ADD(jy, h.tJJ);
+							sLast = s;
+							*dst = m;
+							if (dump)
+								P.dbg_fwd[(size_t)(i - 1)*LY + j0 + lane*C + c] = m;
+							}
+						if (last && i == X.len && lane == g.lcl)    // cell (LX,LY) is the lane's last
+							{
+							float *f = cfin + 5*kp;
+							f[0] = lm; f[1] = ix; f[2] = iy; f[3] = jx; f[4] = jy;
+							}
+						outM = lm; outAIY = laiy; outAJY = lajy; outS = sLast;
+						if (lane == 31 && !last)
+							edgeOut[i] = make_float4(outM, outAIY, outAJY, outS);
+						}
+					else if (i == X.len + 1 && lane < nl)        // separator, then the next pair of the chain
+						{
+						mb_clear_state(st, C, lane);
+						outM = Z; outAIY = Z; outAJY = Z; outS = Z;
+						dprev = Z;
+						if (++kp < nch)
+							{
+							X = mb_seq(P, P.px[cpairs[kp]]);
+							r0 = t + 1;
+							}
+						else
+							r0 = 1 << 30;                 // done: idle for the rest of the strip
+						}
+					}
+				__syncwarp();
+				}
+		else
+			{
+			// Plain mode, two rows per lane per step.  Lane l steps through the pair's rows two at a time, row a
+			// and row b = a+1: row b takes row a's {S, M, IX, JX} of each column from registers, and only row
+			// b's record goes to shared memory.  A pair of even LX starts with row -1, which is all LOG_ZERO
+			// (every input is, and LOG_ZERO is absorbing), so the steps hold rows (LX-1, LX), (LX-3, LX-2), ...
+			// and Backward pairs its rows on the same Forward steps.  After row LX comes one separator step, as
+			// above; pair k starts at chain step Fk + l, Fk = sum over earlier pairs of mb_fwd_steps(LX, 2).
+			for (int strip = 0; strip < g.n; ++strip)
+				{
+				const auto [j0, nl, cn, last] = g.at(strip, lane);
+				const auto [edgeIn, edgeOut] = mb_strip_edges(edge0, edge1, strip);
+				float2 *fms = reinterpret_cast<float2 *>(fm) + (size_t) strip*P.fm_rows*W;   // [step][c][lane] {row a, row b}
+
+				mb_stage_y<false>(Y, j0 + lane*C, C, lane, h.pad, st, ye, y2);
+				float oMa = Z, oIa = Z, oJa = Z, oSa = Z, oMb = Z, oIb = Z, oJb = Z, oSb = Z;
+				float dprev = Z;
+				float bIX = Z, bJX = Z;
+				const int nsteps = sumFS - 2 + nl;
+				int kp = 0, r0 = lane;                // the lane's pair and the step of its first rows
+				MbSeq X = mb_seq(P, P.px[cpairs[0]]);
+				int pad = ~X.len & 1, nq = X.len/2 + 1;   // row -1 or not; the pair's row steps
+				auto xcode = [&](int i) { return i >= 1 && i <= X.len ? (int) X.code[i - 1] : h.pad; };
+				int xa = h.pad, xb = xcode(1 - pad);     // classes of the next step's rows
+				// the left border of row i in lane 0 of strip 0: the start scores at (0,0), the bIX / bJX chain
+				auto border = [&](int i, float ex, float &Lm, float &Laiy, float &Lajy, float &Ls)
+					{
+					Lm = Z;
+					if (i <= 0)
+						{
+						Laiy = i == 0 ? h.tSI : Z; Lajy = i == 0 ? h.tSJ : Z; Ls = i == 0 ? h.tSM : Z;
+						}
+					else
+						{
+						if (i == 1)
+							{
+							bIX = ADD(h.tSI, ex); bJX = ADD(h.tSJ, ex);
 							}
 						else
 							{
-							const float4 e = edgeIn[i];
-							Lm = e.x; Laiy = e.y; Lajy = e.z; Ls = e.w;
+							bIX = ADD(ADD(bIX, h.tII), ex); bJX = ADD(ADD(bJX, h.tJJ), ex);
+							}
+						Laiy = Z; Lajy = Z;
+						Ls = la(ADD(bIX, h.tIM), ADD(bJX, h.tJM));
+						}
+					};
+				for (int t = 0; t < nsteps; ++t)
+					{
+					const int q = t - r0;
+					const int ia = 2*q - pad;             // rows ia and ia+1 of pair kp
+					const int xca = xa, xcb = xb;
+					xa = xcode(ia + 2); xb = xcode(ia + 3);
+					float Lma = __shfl_up_sync(MB_FULL, oMa, 1);
+					float Laiya = __shfl_up_sync(MB_FULL, oIa, 1);
+					float Lajya = __shfl_up_sync(MB_FULL, oJa, 1);
+					float Lsa = __shfl_up_sync(MB_FULL, oSa, 1);
+					float Lmb = __shfl_up_sync(MB_FULL, oMb, 1);
+					float Laiyb = __shfl_up_sync(MB_FULL, oIb, 1);
+					float Lajyb = __shfl_up_sync(MB_FULL, oJb, 1);
+					float Lsb = __shfl_up_sync(MB_FULL, oSb, 1);
+					if (q >= 0 && q < nq && lane < nl)
+						{
+						const float2 *mea = meT + xca*h.KS, *meb = meT + xcb*h.KS;
+						const float exa = sm.insT[xca], exb = sm.insT[xcb];
+						if (lane == 0)
+							{
+							if (strip == 0)
+								{
+								border(ia, exa, Lma, Laiya, Lajya, Lsa);
+								border(ia + 1, exb, Lmb, Laiyb, Lajyb, Lsb);
+								}
+							else
+								{
+								const float4 ea = edgeIn[ia + 1], eb = edgeIn[ia + 2];    // row i at i+1: row -1 too
+								Lma = ea.x; Laiya = ea.y; Lajya = ea.z; Lsa = ea.w;
+								Lmb = eb.x; Laiyb = eb.y; Lajyb = eb.z; Lsb = eb.w;
+								}
+							}
+						float diaga = dprev, diagb = Lsa;
+						dprev = Lsb;
+						float lma = Lma, laiya = Laiya, lajya = Lajya, sLasta = Z;
+						float lmb = Lmb, laiyb = Laiyb, lajyb = Lajyb, sLastb = Z;
+						float ixb = Z, jxb = Z, iyb = Z, jyb = Z;
+						float4 *sp = st + lane;
+						const uint32_t *y2p = y2 + lane;
+						float2 *dst = fms + (size_t) t*W + lane;
+						const bool dump = DUMP && cpairs[kp] == P.dbg_pair;
+#pragma unroll 1
+						for (int c = 0; c < cn; ++c, sp += 32, y2p += 32, dst += 32)
+							{
+							const float4 v = *sp;                      // {S, M, IX, JX} of row a-1
+							const uint32_t yc = *y2p;
+							const float2 ea = mea[yc];                 // {match of row a, insert of Y}
+							const float emb = reinterpret_cast<const float *>(meb + yc)[0];
+							const float eyc = ea.y;
+							const float ma = ADD(diaga, ea.x);
+							const float ixa = ADD(la(ADD(v.z, h.tII), ADD(v.y, h.tMI)), exa);
+							const float jxa = ADD(la(ADD(v.w, h.tJJ), ADD(v.y, h.tMJ)), exa);
+							const float iya = ADD(la(laiya, ADD(lma, h.tMI)), eyc);
+							const float jya = ADD(la(lajya, ADD(lma, h.tMJ)), eyc);
+							const float sa = la(ADD(ma, h.tMM), la(ADD(ixa, h.tIM), la(ADD(jxa, h.tJM),
+							  la(ADD(iya, h.tIM), ADD(jya, h.tJM)))));
+							const float mb = ADD(diagb, emb);
+							ixb = ADD(la(ADD(ixa, h.tII), ADD(ma, h.tMI)), exb);
+							jxb = ADD(la(ADD(jxa, h.tJJ), ADD(ma, h.tMJ)), exb);
+							iyb = ADD(la(laiyb, ADD(lmb, h.tMI)), eyc);
+							jyb = ADD(la(lajyb, ADD(lmb, h.tMJ)), eyc);
+							const float sb = la(ADD(mb, h.tMM), la(ADD(ixb, h.tIM), la(ADD(jxb, h.tJM),
+							  la(ADD(iyb, h.tIM), ADD(jyb, h.tJM)))));
+							diaga = v.x;
+							diagb = sa;
+							*sp = make_float4(sb, mb, ixb, jxb);
+							lma = ma; laiya = ADD(iya, h.tII); lajya = ADD(jya, h.tJJ); sLasta = sa;
+							lmb = mb; laiyb = ADD(iyb, h.tII); lajyb = ADD(jyb, h.tJJ); sLastb = sb;
+							*dst = make_float2(ma, mb);
+							if (dump)
+								{
+								if (ia >= 1)
+									P.dbg_fwd[(size_t)(ia - 1)*LY + j0 + lane*C + c] = ma;
+								if (ia >= 0)
+									P.dbg_fwd[(size_t) ia*LY + j0 + lane*C + c] = mb;
+								}
+							}
+						if (last && ia + 1 == X.len && lane == g.lcl)    // cell (LX,LY): row b, the lane's last
+							{
+							float *f = cfin + 5*kp;
+							f[0] = lmb; f[1] = ixb; f[2] = iyb; f[3] = jxb; f[4] = jyb;
+							}
+						oMa = lma; oIa = laiya; oJa = lajya; oSa = sLasta;
+						oMb = lmb; oIb = laiyb; oJb = lajyb; oSb = sLastb;
+						if (lane == 31 && !last)
+							{
+							edgeOut[ia + 1] = make_float4(oMa, oIa, oJa, oSa);
+							edgeOut[ia + 2] = make_float4(oMb, oIb, oJb, oSb);
 							}
 						}
-					float diag = dprev;
-					dprev = Ls;
-					float lm = Lm, laiy = Laiy, lajy = Lajy, sLast = Z;
-					float ix = Z, jx = Z, iy = Z, jy = Z;
-					float4 *sp = st + lane;
-					const uint2 *yp = ye + lane;
-					const uint32_t *y2p = y2 + lane;
-					float *dst = fms + (size_t) t*W + lane;
-					const bool dump = DUMP && i >= 1 && cpairs[kp] == P.dbg_pair;
-#pragma unroll 1
-					for (int c = 0; c < cn; ++c, sp += 32, yp += 32, y2p += 32, dst += 32)
+					else if (q == nq && lane < nl)        // separator, then the next pair of the chain
 						{
-						const float4 v = *sp;                      // {S, M, IX, JX} of row i-1
-						const auto [em, eyc] = mb_col_emit<MEGA>(matchT, xe, nf, yp, y2p);
-						const float m = ADD(diag, em);
-						ix = ADD(la(ADD(v.z, h.tII), ADD(v.y, h.tMI)), ex);
-						jx = ADD(la(ADD(v.w, h.tJJ), ADD(v.y, h.tMJ)), ex);
-						iy = ADD(la(laiy, ADD(lm, h.tMI)), eyc);
-						jy = ADD(la(lajy, ADD(lm, h.tMJ)), eyc);
-						const float s = la(ADD(m, h.tMM), la(ADD(ix, h.tIM), la(ADD(jx, h.tJM),
-						  la(ADD(iy, h.tIM), ADD(jy, h.tJM)))));
-						diag = v.x;
-						*sp = make_float4(s, m, ix, jx);
-						lm = m;
-						laiy = ADD(iy, h.tII);
-						lajy = ADD(jy, h.tJJ);
-						sLast = s;
-						*dst = m;
-						if (dump)
-							P.dbg_fwd[(size_t)(i - 1)*LY + j0 + lane*C + c] = m;
+						mb_clear_state(st, C, lane);
+						oMa = Z; oIa = Z; oJa = Z; oSa = Z; oMb = Z; oIb = Z; oJb = Z; oSb = Z;
+						dprev = Z;
+						if (++kp < nch)
+							{
+							X = mb_seq(P, P.px[cpairs[kp]]);
+							pad = ~X.len & 1; nq = X.len/2 + 1;
+							r0 = t + 1;
+							xa = h.pad; xb = xcode(1 - pad);
+							}
+						else
+							r0 = 1 << 29;                 // done: idle for the rest of the strip
 						}
-					if (last && i == X.len && lane == g.lcl)    // cell (LX,LY) is the lane's last
-						{
-						float *f = cfin + 5*kp;
-						f[0] = lm; f[1] = ix; f[2] = iy; f[3] = jx; f[4] = jy;
-						}
-					outM = lm; outAIY = laiy; outAJY = lajy; outS = sLast;
-					if (lane == 31 && !last)
-						edgeOut[i] = make_float4(outM, outAIY, outAJY, outS);
 					}
-				else if (i == X.len + 1 && lane < nl)        // separator, then the next pair of the chain
-					{
-					mb_clear_state(st, C, lane);
-					outM = Z; outAIY = Z; outAJY = Z; outS = Z;
-					dprev = Z;
-					if (++kp < nch)
-						{
-						X = mb_seq(P, P.px[cpairs[kp]]);
-						r0 = t + 1;
-						}
-					else
-						r0 = 1 << 30;                 // done: idle for the rest of the strip
-					}
+				__syncwarp();
 				}
-			__syncwarp();
 			}
 
 		// ============================ total probability, lane k for pair k ============================
@@ -708,159 +869,378 @@ k_posterior_sm(const PostParams P)
 		const float keepScore = fmaxf(h.minScore, __uint_as_float(0xc0935d8eu));
 		uint32_t kept = 0;
 		bool overflow = false;
-		for (int strip = g.n - 1; strip >= 0; --strip)
-			{
-			const auto [j0, nl, cn, last] = g.at(strip, lane);
-			const auto [edgeIn, edgeOut] = mb_strip_edges(edge0, edge1, strip);
-			const float *fms = fm + (size_t) strip*P.fm_rows*W;
-
-			mb_stage_y<MEGA>(Y, j0 + lane*C + 1, C, lane, h.pad, st, ye, y2);
-			float outM = Z, outIY = Z, outJY = Z;
-			uint32_t outCnt = 0;
-			float dprev = Z;
-			const int nsteps = sumLX + nch - 2 + nl;
-			int kp = nch - 1, u0 = nl - 1 - lane;   // the lane's pair and the step of its row LX
-			MbSeq X = mb_seq(P, P.px[cpairs[nch - 1]]);
-			MbXRow xPref = mb_x_row<MEGA>(X, false, 0, h.pad);
-			int fk = sumLX - X.len + 2*(nch - 1);   // chain Forward step of the pair's row 0, less the lane
-			int rk = sumLX - X.len;               // chain row of the pair's row 1 in rows / rowcnt
-			float total = ctotal[nch - 1];
-			for (int u = 0; u < nsteps; ++u)
+		if constexpr (R == 1)
+			for (int strip = g.n - 1; strip >= 0; --strip)
 				{
-				const int i = X.len - u + u0;
-				const MbXRow x = xPref;
-				xPref = mb_x_row<MEGA>(X, i >= 2 && i <= X.len, i - 1, h.pad);
-				float Rm = __shfl_down_sync(MB_FULL, outM, 1);
-				float Riy = __shfl_down_sync(MB_FULL, outIY, 1);
-				float Rjy = __shfl_down_sync(MB_FULL, outJY, 1);
-				uint32_t cnt = __shfl_down_sync(MB_FULL, outCnt, 1);    // entries already in the row
-				if (i >= 1 && i <= X.len && lane < nl)
+				const auto [j0, nl, cn, last] = g.at(strip, lane);
+				const auto [edgeIn, edgeOut] = mb_strip_edges(edge0, edge1, strip);
+				const float *fms = fm + (size_t) strip*P.fm_rows*W;
+
+				mb_stage_y<MEGA>(Y, j0 + lane*C + 1, C, lane, h.pad, st, ye, y2);
+				float outM = Z, outIY = Z, outJY = Z;
+				uint32_t outCnt = 0;
+				float dprev = Z;
+				const int nsteps = sumLX + nch - 2 + nl;
+				int kp = nch - 1, u0 = nl - 1 - lane;   // the lane's pair and the step of its row LX
+				MbSeq X = mb_seq(P, P.px[cpairs[nch - 1]]);
+				MbXRow xPref = mb_x_row<MEGA>(X, false, 0, h.pad);
+				int fk = sumLX - X.len + 2*(nch - 1);   // chain Forward step of the pair's row 0, less the lane
+				int rk = sumLX - X.len;               // chain row of the pair's row 1 in rows / rowcnt
+				float total = ctotal[nch - 1];
+				for (int u = 0; u < nsteps; ++u)
 					{
-					if (lane == nl - 1)
+					const int i = X.len - u + u0;
+					const MbXRow x = xPref;
+					xPref = mb_x_row<MEGA>(X, i >= 2 && i <= X.len, i - 1, h.pad);
+					float Rm = __shfl_down_sync(MB_FULL, outM, 1);
+					float Riy = __shfl_down_sync(MB_FULL, outIY, 1);
+					float Rjy = __shfl_down_sync(MB_FULL, outJY, 1);
+					uint32_t cnt = __shfl_down_sync(MB_FULL, outCnt, 1);    // entries already in the row
+					if (i >= 1 && i <= X.len && lane < nl)
 						{
-						if (last)
+						if (lane == nl - 1)
 							{
-							Rm = Z; Riy = Z; Rjy = Z; cnt = 0;
+							if (last)
+								{
+								Rm = Z; Riy = Z; Rjy = Z; cnt = 0;
+								}
+							else
+								{
+								const float4 e = edgeIn[i];
+								Rm = e.x; Riy = e.y; Rjy = e.z; cnt = __float_as_uint(e.w);
+								}
 							}
-						else
+						const MbXEmit xe = mb_x_emit<MEGA>(P, sm.insT, meT, h.KS, x);
+						const float ex = xe.ins;
+						const int t = fk + i + lane;
+						const int col0 = j0 + lane*C;
+						float mdiag = dprev;
+						dprev = Rm;
+						float riy = Riy, rjy = Rjy, mFirst = Z;
+						// posterior score (calcposteriorflat.cpp:14-22) and its threshold; columns arrive descending,
+						// so bit c of hits ends up on column c
+						uint32_t hits = 0;
+						auto post = [&](int c, float fmv, float m)
 							{
-							const float4 e = edgeIn[i];
-							Rm = e.x; Riy = e.y; Rjy = e.z; cnt = __float_as_uint(e.w);
-							}
-						}
-					const MbXEmit xe = mb_x_emit<MEGA>(P, sm.insT, meT, h.KS, x);
-					const float ex = xe.ins;
-					const int t = fk + i + lane;
-					const int col0 = j0 + lane*C;
-					float mdiag = dprev;
-					dprev = Rm;
-					float riy = Riy, rjy = Rjy, mFirst = Z;
-					// posterior score (calcposteriorflat.cpp:14-22) and its threshold; columns arrive descending,
-					// so bit c of hits ends up on column c
-					uint32_t hits = 0;
-					auto post = [&](int c, float fmv, float m)
-						{
-						const float score = __fsub_rn(ADD(fmv, m), total);
-						hits = 2u*hits + (score >= h.minScore ? 1u : 0u);
-						if (DUMP && cpairs[kp] == P.dbg_pair)
+							const float score = __fsub_rn(ADD(fmv, m), total);
+							hits = 2u*hits + (score >= h.minScore ? 1u : 0u);
+							if (DUMP && cpairs[kp] == P.dbg_pair)
+								{
+								P.dbg_bwd[(size_t)(i - 1)*LY + col0 + c] = m;
+								P.dbg_post[(size_t)(i - 1)*LY + col0 + c] =
+								  score < h.minScore ? 0.0f : (score >= 0.0f ? 1.0f : mb_expf_glibc(score));
+								}
+							return score;
+							};
+						float4 *sp = st + lane;
+						const uint2 *yp = ye + lane;
+						const uint32_t *y2p = y2 + lane;
+						const float *src = fms + (size_t) t*W + lane;     // Forward M of the lane's column 0
+						int c = cn - 1;
+						sp += c*32; yp += c*32; y2p += c*32; src += c*32;
+						if (last && i == X.len && lane == g.lcl)
 							{
-							P.dbg_bwd[(size_t)(i - 1)*LY + col0 + c] = m;
-							P.dbg_post[(size_t)(i - 1)*LY + col0 + c] =
-							  score < h.minScore ? 0.0f : (score >= 0.0f ? 1.0f : mb_expf_glibc(score));
+							// cell (LX,LY), the lane's first: the end scores (bwdflat3.cpp:53-61)
+							mdiag = sp->x;
+							*sp = make_float4(h.tSM, h.tSI, h.tSJ, post(c, *src, h.tSM));
+							riy = h.tSI; rjy = h.tSJ; mFirst = h.tSM;
+							--c; sp -= 32; yp -= 32; y2p -= 32; src -= 32;
 							}
-						return score;
-						};
-					float4 *sp = st + lane;
-					const uint2 *yp = ye + lane;
-					const uint32_t *y2p = y2 + lane;
-					const float *src = fms + (size_t) t*W + lane;     // Forward M of the lane's column 0
-					int c = cn - 1;
-					sp += c*32; yp += c*32; y2p += c*32; src += c*32;
-					if (last && i == X.len && lane == g.lcl)
-						{
-						// cell (LX,LY), the lane's first: the end scores (bwdflat3.cpp:53-61)
-						mdiag = sp->x;
-						*sp = make_float4(h.tSM, h.tSI, h.tSJ, post(c, *src, h.tSM));
-						riy = h.tSI; rjy = h.tSJ; mFirst = h.tSM;
-						--c; sp -= 32; yp -= 32; y2p -= 32; src -= 32;
-						}
-					// Forward M is loaded two columns ahead.  ptxas places the load where register pressure lets
-					// it, mid-loop here; one column ahead that left less than an iteration to cover an HBM miss and
-					// cost C4 6 % (the CM = 16 class runs 4 warps per scheduler).  The loads stay within this step's
-					// columns, except *src when the cell (LX,LY) was the lane's only column (c = -1): that is
-					// step t-1's column C-1 (t is the same in every lane), inside this warp's spill since t >= 1
-					float fmNext = *src;                       // column c
-					float fmNext2 = c >= 1 ? src[-32] : 0.0f;  // column c-1
+						// Forward M is loaded two columns ahead.  ptxas places the load where register pressure lets
+						// it, mid-loop here; one column ahead that left less than an iteration to cover an HBM miss and
+						// cost C4 6 % (the CM = 16 class runs 4 warps per scheduler).  The loads stay within this step's
+						// columns, except *src when the cell (LX,LY) was the lane's only column (c = -1): that is
+						// step t-1's column C-1 (t is the same in every lane), inside this warp's spill since t >= 1
+						float fmNext = *src;                       // column c
+						float fmNext2 = c >= 1 ? src[-32] : 0.0f;  // column c-1
 #pragma unroll 1
-					for (; c >= 0; --c, sp -= 32, yp -= 32, y2p -= 32)
-						{
-						const float fmv = fmNext;
-						fmNext = fmNext2;
-						src -= 32;
-						if (c >= 2)
-							fmNext2 = src[-32];                // column c-2
-						const float4 v = *sp;                      // {M, IX, JX, score} of row i+1
-						const auto [em, eyc] = mb_col_emit<MEGA>(matchT, xe, nf, yp, y2p);
-						const float nM = ADD(mdiag, em);
-						const float nIX = ADD(v.y, ex);
-						const float nJX = ADD(v.z, ex);
-						const float nIY = ADD(riy, eyc);
-						const float nJY = ADD(rjy, eyc);
-						const float m = la(ADD(h.tMM, nM), la(ADD(h.tMI, nIX), la(ADD(h.tMJ, nJX),
-						  la(ADD(h.tMI, nIY), ADD(h.tMJ, nJY)))));
-						const float ix = la(ADD(h.tII, nIX), ADD(h.tIM, nM));
-						const float jx = la(ADD(h.tJJ, nJX), ADD(h.tJM, nM));
-						const float iy = la(ADD(h.tII, nIY), ADD(h.tIM, nM));
-						const float jy = la(ADD(h.tJJ, nJY), ADD(h.tJM, nM));
-						mdiag = v.x;
-						*sp = make_float4(m, ix, jx, post(c, fmv, m));
-						riy = iy; rjy = jy;
-						mFirst = m;
+						for (; c >= 0; --c, sp -= 32, yp -= 32, y2p -= 32)
+							{
+							const float fmv = fmNext;
+							fmNext = fmNext2;
+							src -= 32;
+							if (c >= 2)
+								fmNext2 = src[-32];                // column c-2
+							const float4 v = *sp;                      // {M, IX, JX, score} of row i+1
+							const auto [em, eyc] = mb_col_emit<MEGA>(matchT, xe, nf, yp, y2p);
+							const float nM = ADD(mdiag, em);
+							const float nIX = ADD(v.y, ex);
+							const float nJX = ADD(v.z, ex);
+							const float nIY = ADD(riy, eyc);
+							const float nJY = ADD(rjy, eyc);
+							const float m = la(ADD(h.tMM, nM), la(ADD(h.tMI, nIX), la(ADD(h.tMJ, nJX),
+							  la(ADD(h.tMI, nIY), ADD(h.tMJ, nJY)))));
+							const float ix = la(ADD(h.tII, nIX), ADD(h.tIM, nM));
+							const float jx = la(ADD(h.tJJ, nJX), ADD(h.tJM, nM));
+							const float iy = la(ADD(h.tII, nIY), ADD(h.tIM, nM));
+							const float jy = la(ADD(h.tJJ, nJY), ADD(h.tJM, nM));
+							mdiag = v.x;
+							*sp = make_float4(m, ix, jx, post(c, fmv, m));
+							riy = iy; rjy = jy;
+							mFirst = m;
+							}
+						// the survivors, highest column first (the row's order): the warp runs this loop as often as
+						// the most survivors in one lane, not once per column in which any lane has one
+						mb200_entry *row = rows + (size_t)(rk + i - 1)*MB_CAP;
+						while (hits)
+							{
+							const int hc = 31 - __clz(hits);
+							hits ^= 1u << hc;
+							const float score = st[hc*32 + lane].w;
+							if (cnt < MB_CAP)
+								*reinterpret_cast<uint2 *>(row + cnt) = make_uint2(__float_as_uint(score), (uint32_t)(col0 + hc));
+							else
+								overflow = true;
+							++cnt;
+							kept += score >= keepScore ? 1u : 0u;
+							}
+						outM = mFirst; outIY = riy; outJY = rjy;
+						outCnt = cnt;
+						if (lane == 0)
+							{
+							if (strip > 0)
+								edgeOut[i] = make_float4(outM, outIY, outJY, __uint_as_float(cnt));
+							else
+								rowcnt[rk + i - 1] = (uint8_t) min(cnt, (uint32_t) MB_CAP);
+							}
 						}
-					// the survivors, highest column first (the row's order): the warp runs this loop as often as
-					// the most survivors in one lane, not once per column in which any lane has one
-					mb200_entry *row = rows + (size_t)(rk + i - 1)*MB_CAP;
-					while (hits)
+					else if (i == 0 && lane < nl)         // separator, then the previous pair of the chain
 						{
-						const int hc = 31 - __clz(hits);
-						hits ^= 1u << hc;
-						const float score = st[hc*32 + lane].w;
-						if (cnt < MB_CAP)
-							*reinterpret_cast<uint2 *>(row + cnt) = make_uint2(__float_as_uint(score), (uint32_t)(col0 + hc));
+						mb_clear_state(st, C, lane);
+						outM = Z; outIY = Z; outJY = Z;
+						outCnt = 0;
+						dprev = Z;
+						ckept[kp*32 + lane] = kept;
+						if (kp > 0)
+							{
+							X = mb_seq(P, P.px[cpairs[--kp]]);
+							u0 = u + 1;
+							fk -= X.len + 2;
+							rk -= X.len;
+							total = ctotal[kp];
+							}
 						else
-							overflow = true;
-						++cnt;
-						kept += score >= keepScore ? 1u : 0u;
+							u0 = -(1 << 30);              // done: idle for the rest of the strip
 						}
-					outM = mFirst; outIY = riy; outJY = rjy;
-					outCnt = cnt;
-					if (lane == 0)
-						{
-						if (strip > 0)
-							edgeOut[i] = make_float4(outM, outIY, outJY, __uint_as_float(cnt));
-						else
-							rowcnt[rk + i - 1] = (uint8_t) min(cnt, (uint32_t) MB_CAP);
-						}
+					__syncwarp();
 					}
-				else if (i == 0 && lane < nl)         // separator, then the previous pair of the chain
+				}
+		else
+			{
+			// Plain mode, two rows per lane per step: row a and row b = a-1, paired on the Forward steps (row a
+			// is a Forward row b), from row LX down, so that the end scores at (LX,LY) are always row a's.  Row b
+			// takes row a's {M, IX, JX} of each column from registers; the record stores row b's and, in the
+			// spare .w, row a's score; a survivor of row b gets its score formed again after the loop from the
+			// stored M and the Forward-M line.  The hits of both rows share one mask (row a in bits 0-15, row b
+			// in 16-31) and their counts one shuffled word.  A pair takes mb_fwd_steps(LX, 2) - 1 steps; when LX
+			// is odd, its last row b is row 0, computed and dropped: the separator ends that step.
+			for (int strip = g.n - 1; strip >= 0; --strip)
+				{
+				const auto [j0, nl, cn, last] = g.at(strip, lane);
+				const auto [edgeIn, edgeOut] = mb_strip_edges(edge0, edge1, strip);
+				const float2 *fms = reinterpret_cast<const float2 *>(fm) + (size_t) strip*P.fm_rows*W;
+
+				mb_stage_y<false>(Y, j0 + lane*C + 1, C, lane, h.pad, st, ye, y2);
+				float oMa = Z, oIa = Z, oJa = Z, oMb = Z, oIb = Z, oJb = Z;
+				uint32_t oCnt = 0;                    // entries already in row a (bits 0-15) and row b (16-31)
+				float dprev = Z;
+				const int nsteps = sumFS - nch - 1 + nl;
+				int kp = nch - 1, u0 = nl - 1 - lane;   // the lane's pair and the step of its row LX
+				MbSeq X = mb_seq(P, P.px[cpairs[nch - 1]]);
+				int pad = ~X.len & 1;
+				int fk = sumFS - (int) mb_fwd_steps(X.len, 2);   // chain Forward step of the pair's first rows, less the lane
+				int rk = sumLX - X.len;               // chain row of the pair's row 1 in rows / rowcnt
+				float total = ctotal[nch - 1];
+				auto xcode = [&](int i) { return i >= 1 && i < X.len ? (int) X.code[i] : h.pad; };   // row i reads residue i+1
+				int xa = h.pad, xb = xcode(X.len - 1);   // classes of the next step's rows
+				// then the previous pair of the chain.  The step's outputs stay: when row b is row 0, lane l-1 still
+				// reads row a's next step (a whole separator step ignores them)
+				auto separator = [&](int u)
 					{
 					mb_clear_state(st, C, lane);
-					outM = Z; outIY = Z; outJY = Z;
-					outCnt = 0;
 					dprev = Z;
 					ckept[kp*32 + lane] = kept;
 					if (kp > 0)
 						{
 						X = mb_seq(P, P.px[cpairs[--kp]]);
 						u0 = u + 1;
-						fk -= X.len + 2;
+						pad = ~X.len & 1;
+						fk -= mb_fwd_steps(X.len, 2);
 						rk -= X.len;
 						total = ctotal[kp];
+						xa = h.pad; xb = xcode(X.len - 1);
 						}
 					else
-						u0 = -(1 << 30);              // done: idle for the rest of the strip
+						u0 = -(1 << 29);              // done: idle for the rest of the strip
+					};
+				for (int u = 0; u < nsteps; ++u)
+					{
+					const int ia = X.len - 2*(u - u0);   // rows ia and ia-1 of pair kp
+					const int xca = xa, xcb = xb;
+					xa = xcode(ia - 2); xb = xcode(ia - 3);
+					float Rma = __shfl_down_sync(MB_FULL, oMa, 1);
+					float Riya = __shfl_down_sync(MB_FULL, oIa, 1);
+					float Rjya = __shfl_down_sync(MB_FULL, oJa, 1);
+					float Rmb = __shfl_down_sync(MB_FULL, oMb, 1);
+					float Riyb = __shfl_down_sync(MB_FULL, oIb, 1);
+					float Rjyb = __shfl_down_sync(MB_FULL, oJb, 1);
+					uint32_t cnt = __shfl_down_sync(MB_FULL, oCnt, 1);
+					if (ia >= 1 && ia <= X.len && lane < nl)
+						{
+						if (lane == nl - 1)
+							{
+							if (last)
+								{
+								Rma = Z; Riya = Z; Rjya = Z; Rmb = Z; Riyb = Z; Rjyb = Z; cnt = 0;
+								}
+							else
+								{
+								const float4 ea = edgeIn[ia], eb = edgeIn[ia - 1];
+								Rma = ea.x; Riya = ea.y; Rjya = ea.z;
+								Rmb = eb.x; Riyb = eb.y; Rjyb = eb.z;
+								cnt = __float_as_uint(ea.w) | __float_as_uint(eb.w) << 16;
+								}
+							}
+						const float2 *mea = meT + xca*h.KS, *meb = meT + xcb*h.KS;
+						const float exa = sm.insT[xca], exb = sm.insT[xcb];
+						const int t = fk + (ia + pad - 1)/2 + lane;   // the Forward step of rows ia-1, ia
+						const int col0 = j0 + lane*C;
+						float mdiaga = dprev, mdiagb = Rma;
+						dprev = Rmb;
+						float riya = Riya, rjya = Rjya, riyb = Riyb, rjyb = Rjyb, mFirsta = Z, mFirstb = Z;
+						// posterior scores (calcposteriorflat.cpp:14-22) and their threshold; columns arrive descending,
+						// so bit c of hits ends up on row a's column c and bit 16+c on row b's
+						uint32_t hits = 0;
+						auto post = [&](int i, int c, float fmv, float m)
+							{
+							const float score = __fsub_rn(ADD(fmv, m), total);
+							if (DUMP && i >= 1 && cpairs[kp] == P.dbg_pair)
+								{
+								P.dbg_bwd[(size_t)(i - 1)*LY + col0 + c] = m;
+								P.dbg_post[(size_t)(i - 1)*LY + col0 + c] =
+								  score < h.minScore ? 0.0f : (score >= 0.0f ? 1.0f : mb_expf_glibc(score));
+								}
+							return score;
+							};
+						// Backward cell from the row below ({M, IX, JX} of this column and M of the next one) and the
+						// IY / JY of the cell to the right
+						auto cell = [&](float mdiag, float vIX, float vJX, float riy, float rjy, float em, float eyc, float ex)
+							{
+							const float nM = ADD(mdiag, em);
+							const float nIX = ADD(vIX, ex);
+							const float nJX = ADD(vJX, ex);
+							const float nIY = ADD(riy, eyc);
+							const float nJY = ADD(rjy, eyc);
+							MbBwdCell r;
+							r.m = la(ADD(h.tMM, nM), la(ADD(h.tMI, nIX), la(ADD(h.tMJ, nJX),
+							  la(ADD(h.tMI, nIY), ADD(h.tMJ, nJY)))));
+							r.ix = la(ADD(h.tII, nIX), ADD(h.tIM, nM));
+							r.jx = la(ADD(h.tJJ, nJX), ADD(h.tJM, nM));
+							r.iy = la(ADD(h.tII, nIY), ADD(h.tIM, nM));
+							r.jy = la(ADD(h.tJJ, nJY), ADD(h.tJM, nM));
+							return r;
+							};
+						float4 *sp = st + lane;
+						const uint32_t *y2p = y2 + lane;
+						const float2 *fmc = fms + (size_t) t*W + lane;   // Forward M {row ia-1, row ia} of the lane's column 0
+						const float2 *src = fmc;
+						int c = cn - 1;
+						sp += c*32; y2p += c*32; src += c*32;
+						if (last && ia == X.len && lane == g.lcl)
+							{
+							// cell (LX,LY), row a's first: the end scores (bwdflat3.cpp:53-61); row b's cell below it
+							const float2 f = *src;
+							const uint32_t yc = *y2p;
+							const float2 e = meb[yc];
+							const float sa = post(ia, c, f.y, h.tSM);
+							const MbBwdCell b = cell(mdiagb, h.tSI, h.tSJ, riyb, rjyb, e.x, e.y, exb);
+							const float sb = post(ia - 1, c, f.x, b.m);
+							hits = (sa >= h.minScore ? 1u : 0u) + (sb >= h.minScore ? 0x10000u : 0u);
+							mdiaga = sp->x;
+							mdiagb = h.tSM;
+							*sp = make_float4(b.m, b.ix, b.jx, sa);
+							riya = h.tSI; rjya = h.tSJ; mFirsta = h.tSM;
+							riyb = b.iy; rjyb = b.jy; mFirstb = b.m;
+							--c; sp -= 32; y2p -= 32; src -= 32;
+							}
+						// Forward M is loaded two columns ahead, as in the single-row loop, and never outside this
+						// step's columns
+						float2 fmNext = c >= 0 ? src[0] : make_float2(0.0f, 0.0f);      // column c
+						float2 fmNext2 = c >= 1 ? src[-32] : make_float2(0.0f, 0.0f);   // column c-1
+#pragma unroll 1
+						for (; c >= 0; --c, sp -= 32, y2p -= 32)
+							{
+							const float2 f = fmNext;
+							fmNext = fmNext2;
+							src -= 32;
+							if (c >= 2)
+								fmNext2 = src[-32];                // column c-2
+							const float4 v = *sp;                      // {M, IX, JX, -} of row ia+1
+							const uint32_t yc = *y2p;
+							const float2 e = mea[yc];                  // {match of row a, insert of Y}
+							const float emb = reinterpret_cast<const float *>(meb + yc)[0];
+							const MbBwdCell a = cell(mdiaga, v.y, v.z, riya, rjya, e.x, e.y, exa);
+							const float sa = post(ia, c, f.y, a.m);
+							const MbBwdCell b = cell(mdiagb, a.ix, a.jx, riyb, rjyb, emb, e.y, exb);
+							const float sb = post(ia - 1, c, f.x, b.m);
+							hits = 2u*hits + (sa >= h.minScore ? 1u : 0u) + (sb >= h.minScore ? 0x10000u : 0u);
+							mdiaga = v.x;
+							mdiagb = a.m;
+							*sp = make_float4(b.m, b.ix, b.jx, sa);
+							riya = a.iy; rjya = a.jy; mFirsta = a.m;
+							riyb = b.iy; rjyb = b.jy; mFirstb = b.m;
+							}
+						// the survivors, row b's then row a's, highest column first (each row's order)
+						if (ia == 1)
+							hits &= 0xffffu;                   // row b is row 0, the separator
+						uint32_t cnta = cnt & 0xffffu, cntb = cnt >> 16;
+						mb200_entry *rowa = rows + (size_t)(rk + ia - 1)*MB_CAP;
+						while (hits)
+							{
+							const int hb = 31 - __clz(hits);
+							hits ^= 1u << hb;
+							const bool inb = hb >= 16;
+							const int hc = hb & 15;
+							const float4 r = st[hc*32 + lane];
+							const float score = inb ? __fsub_rn(ADD(fmc[hc*32].x, r.x), total) : r.w;
+							const uint32_t n = inb ? cntb : cnta;
+							if (n < MB_CAP)
+								*reinterpret_cast<uint2 *>(rowa - (inb ? MB_CAP : 0) + n) =
+								  make_uint2(__float_as_uint(score), (uint32_t)(col0 + hc));
+							else
+								overflow = true;
+							if (inb)
+								++cntb;
+							else
+								++cnta;
+							kept += score >= keepScore ? 1u : 0u;
+							}
+						cnta = min(cnta, (uint32_t) MB_CAP);
+						cntb = min(cntb, (uint32_t) MB_CAP);
+						oMa = mFirsta; oIa = riya; oJa = rjya;
+						oMb = mFirstb; oIb = riyb; oJb = rjyb;
+						oCnt = cnta | cntb << 16;
+						if (lane == 0)
+							{
+							if (strip > 0)
+								{
+								edgeOut[ia] = make_float4(oMa, oIa, oJa, __uint_as_float(cnta));
+								edgeOut[ia - 1] = make_float4(oMb, oIb, oJb, __uint_as_float(cntb));
+								}
+							else
+								{
+								rowcnt[rk + ia - 1] = (uint8_t) cnta;
+								if (ia > 1)
+									rowcnt[rk + ia - 2] = (uint8_t) cntb;
+								}
+							}
+						if (ia == 1)
+							separator(u);
+						}
+					else if (ia == 0 && lane < nl)
+						separator(u);
+					__syncwarp();
 					}
-				__syncwarp();
 				}
 			}
 		ckept[lane] = kept;                       // the end of pair 0 (its separator may lie past the last step)
