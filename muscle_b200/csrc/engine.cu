@@ -125,7 +125,7 @@ void mb200_destroy(mb200_ctx *ctx)
 	  &ctx->d_py, &ctx->d_order, &ctx->d_chain,
 	  &ctx->d_rowoff, &ctx->d_rowbase, &ctx->d_entries, &ctx->d_cursor, &ctx->d_entbase, &ctx->d_nnz,
 	  &ctx->d_ea, &ctx->d_dbg, &ctx->d_pack_off, &ctx->d_pack_ent, &ctx->d_entries2,
-	  &ctx->d_tr_rowoff, &ctx->d_tr_rowbase, &ctx->d_tr_entries, &ctx->d_tr_entbase, &ctx->d_tr_perm,
+	  &ctx->d_tr_rowoff, &ctx->d_tr_rowbase, &ctx->d_tr_entries, &ctx->d_tr_perm,
 	  &ctx->d_tmp, &ctx->d_tmp2, &ctx->d_mk_hdr, &ctx->d_mk_words, &ctx->d_tr_mk_hdr, &ctx->d_tr_mk_words,
 	  &ctx->d_relax_order, &ctx->d_p2c, &ctx->d_join, &ctx->d_stage, &ctx->d_megaT, &ctx->d_insP };
 	if (ctx->h_pinned)
@@ -392,57 +392,23 @@ int mb200_set_seqs_mega(mb200_ctx *ctx, uint32_t nseq, const uint8_t *letters, c
 // Forward-M spill and candidate rows: at 1280 the C3 workload (1000 proteins of ~350 residues) runs
 // chains of about 3.5 pairs and its scratch stays a small part of one 80 GB device.
 static const uint64_t kChainRows = 1280;
-// Plan = everything that depends only on the pair list: per-pair row bases, the column-width
-// bins and the longest-first work order.  Cached across calls with the same pair list so that a
-// repeated mb200_posteriors_allpairs() moves no host data.
-static int prepare_plan(mb200_ctx *ctx, int force_c)
+// The plan of the installed pair list (PostPlan, engine.h): the column-width bins and, inside each, the
+// chains in longest-first work order.  Cached across calls with the same pair list so that a repeated
+// mb200_posteriors_allpairs() moves no host data.
+static int build_plan(mb200_ctx *ctx, int force_c, int R)
 	{
 	const uint32_t np = (uint32_t) ctx->h_px.size();
-	cudaStream_t st = ctx->stream;
-	std::vector<uint64_t> rowbase(np + 1);
-	uint64_t cells = 0, rows_total = 0, est_entries = 0;
-	// per-pair geometry, reference overflow guard (fwdflat3.cpp:17-18)
+	PostPlan &plan = ctx->plan;
+	plan = PostPlan{};
+	// reference overflow guard (fwdflat3.cpp:17-18); bin pairs by C = columns per lane
+	std::vector<std::vector<uint32_t>> bins(MB_MAX_C + 1);
 	for (uint32_t k = 0; k < np; ++k)
 		{
-		const uint32_t x = ctx->h_px[k], y = ctx->h_py[k];
-		if (x >= ctx->nseq || y >= ctx->nseq)
-			return mb_fail(ctx, MB200_EINVAL, "pair %u references sequence out of range", k);
-		const double LX = ctx->h_len[x], LY = ctx->h_len[y];
-		if (LX*LY*5 + 100 > 2147483647.0)
-			return mb_fail(ctx, MB200_EOVERFLOW, "HMM overflow, sequence lengths %u, %u (max ~21k)",
-			  ctx->h_len[x], ctx->h_len[y]);
-		rowbase[k] = rows_total;
-		rows_total += ctx->h_len[x] + 1;
-		cells += (uint64_t) ctx->h_len[x]*ctx->h_len[y];
-		est_entries += (uint64_t) ctx->h_len[x]*ctx->nnz_per_row_cap;
-		}
-	rowbase[np] = rows_total;
-	ctx->h_rowbase = rowbase;
-	ctx->plan_cells = cells;
-	ctx->plan_est_entries = est_entries;
-
-	ENSURE(ctx->d_px, np*sizeof(uint32_t));
-	ENSURE(ctx->d_py, np*sizeof(uint32_t));
-	ENSURE(ctx->d_rowbase, (np + 1)*sizeof(uint64_t));
-	ENSURE(ctx->d_rowoff, rows_total*sizeof(uint32_t));
-	ENSURE(ctx->d_entbase, np*sizeof(uint64_t));
-	ENSURE(ctx->d_nnz, np*sizeof(uint32_t));
-	ENSURE(ctx->d_ea, np*sizeof(float));
-	ENSURE(ctx->d_order, np*sizeof(uint32_t));
-	// one control block = { entry cursor u64, error flag i32, pad, work cursors u32[MB_MAX_C+1] }:
-	// a single memset per step and a single 16-byte read-back
-	ENSURE(ctx->d_cursor, 16 + (MB_MAX_C + 1)*sizeof(uint32_t));
-	CU(cudaMemcpyAsync(ctx->d_px.p, ctx->h_px.data(), np*sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(ctx->d_py.p, ctx->h_py.data(), np*sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(ctx->d_rowbase.p, rowbase.data(), (np + 1)*sizeof(uint64_t), cudaMemcpyHostToDevice, st));
-	ctx->stats.h2d_bytes += 2ull*np*sizeof(uint32_t) + (np + 1)*sizeof(uint64_t);
-
-	// bin pairs by C = columns per lane
-	auto &bins = ctx->plan_bins;
-	bins.assign(MB_MAX_C + 1, std::vector<uint32_t>());
-	for (uint32_t k = 0; k < np; ++k)
-		{
-		const uint32_t LY = ctx->h_len[ctx->h_py[k]];
+		const uint32_t LX = ctx->h_len[ctx->h_px[k]], LY = ctx->h_len[ctx->h_py[k]];
+		if ((double) LX*LY*5 + 100 > 2147483647.0)
+			return mb_fail(ctx, MB200_EOVERFLOW, "HMM overflow, sequence lengths %u, %u (max ~21k)", LX, LY);
+		plan.cells += (uint64_t) LX*LY;
+		plan.est_entries += (uint64_t) LX*ctx->nnz_per_row_cap;
 		int C = force_c > 0 ? force_c : (int) std::min<uint32_t>(MB_MAX_C, (LY + 31)/32);
 		if (force_c <= 0)
 			C = mb_post_sm_class(C);          // bins only size the shared-memory state
@@ -452,15 +418,10 @@ static int prepare_plan(mb200_ctx *ctx, int force_c)
 	// MB_CHAIN_MAX pairs; pairs that need more than one strip stay alone); most cells first
 	std::vector<uint32_t> order, chain;
 	order.reserve(np);
-	ctx->plan_bin_start.assign(MB_MAX_C + 2, 0);
-	ctx->plan_lxmax.assign(MB_MAX_C + 1, 0);
-	ctx->plan_lymax.assign(MB_MAX_C + 1, 0);
-	ctx->plan_fmax.assign(MB_MAX_C + 1, 0);
-	ctx->plan_fsteps.assign(MB_MAX_C + 1, 0);
-	ctx->plan_rmax.assign(MB_MAX_C + 1, 0);
 	std::vector<int> open(ctx->nseq, -1);
 	for (int C = 1; C <= MB_MAX_C; ++C)
 		{
+		PostClass &pc = plan.cls[C];
 		std::vector<std::vector<uint32_t>> chains;
 		std::vector<uint64_t> frows, fsteps, cost;
 		for (uint32_t k : bins[C])
@@ -478,184 +439,198 @@ static int prepare_plan(mb200_ctx *ctx, int force_c)
 				}
 			chains[c].push_back(k);
 			frows[c] += LX + 2;
-			fsteps[c] += mb_fwd_steps(LX, MB_PLAIN_ROWS);
+			fsteps[c] += mb_fwd_steps(LX, R);
 			cost[c] += (uint64_t) LX*LY;
-			ctx->plan_lxmax[C] = std::max(ctx->plan_lxmax[C], LX);
-			ctx->plan_lymax[C] = std::max(ctx->plan_lymax[C], LY);
-			ctx->plan_fmax[C] = std::max<uint64_t>(ctx->plan_fmax[C], frows[c]);
-			ctx->plan_fsteps[C] = std::max<uint64_t>(ctx->plan_fsteps[C], fsteps[c]);
-			ctx->plan_rmax[C] = std::max<uint64_t>(ctx->plan_rmax[C], frows[c] - 2*chains[c].size());
+			pc.lxmax = std::max(pc.lxmax, LX);
+			pc.lymax = std::max(pc.lymax, LY);
+			pc.fsteps = std::max<uint64_t>(pc.fsteps, fsteps[c]);
+			pc.rows = std::max<uint64_t>(pc.rows, frows[c] - 2*chains[c].size());
 			}
 		for (uint32_t k : bins[C])
 			open[ctx->h_py[k]] = -1;
 		std::vector<uint32_t> idx(chains.size());
 		std::iota(idx.begin(), idx.end(), 0u);
 		std::stable_sort(idx.begin(), idx.end(), [&](uint32_t a, uint32_t b) { return cost[a] > cost[b]; });
-		ctx->plan_bin_start[C] = (uint32_t) chain.size();
+		pc.chain0 = (uint32_t) chain.size();
+		pc.nchains = (uint32_t) chains.size();
 		for (uint32_t c : idx)
 			{
 			chain.push_back((uint32_t) order.size());
 			order.insert(order.end(), chains[c].begin(), chains[c].end());
 			}
 		}
-	ctx->plan_bin_start[MB_MAX_C + 1] = (uint32_t) chain.size();
 	chain.push_back((uint32_t) order.size());
+	cudaStream_t st = ctx->stream;
 	ENSURE(ctx->d_chain, chain.size()*sizeof(uint32_t));
+	ENSURE(ctx->d_order, np*sizeof(uint32_t));
 	CU(cudaMemcpyAsync(ctx->d_chain.p, chain.data(), chain.size()*sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-	ctx->stats.h2d_bytes += chain.size()*sizeof(uint32_t);
 	CU(cudaMemcpyAsync(ctx->d_order.p, order.data(), np*sizeof(uint32_t), cudaMemcpyHostToDevice, st));
 	CU(cudaStreamSynchronize(st));     // host vectors above go out of scope
-	ctx->stats.h2d_bytes += np*sizeof(uint32_t);
-	ctx->plan_valid = true;
-	ctx->plan_force_c = force_c;
+	ctx->stats.h2d_bytes += chain.size()*sizeof(uint32_t) + np*sizeof(uint32_t);
+	plan.valid = true;
+	plan.force_c = force_c;
+	plan.R = R;
 	return MB200_OK;
 	}
 
+// one launch of k_posterior_sm: the size class's instantiation, its dynamic shared memory and grid
+struct ClassLaunch { const void *kern; size_t smem; uint32_t nblocks; PostParams P; };
+
+// The launch of size class C with an entry pool of ent_cap entries.  Its per-warp scratch is one buffer
+// whose warp count shrinks to fit 80 % of the free memory; free_b is that free memory, 0 = not known
+// (it is asked for, and reset when a scratch buffer is (re)allocated).
+static int class_launch(mb200_ctx *ctx, int C, const PostDebug *dbg, uint64_t ent_cap, size_t &free_b, ClassLaunch &L)
+	{
+	const PostClass &pc = ctx->plan.cls[C];
+	const bool mega = ctx->mega;
+	const bool dump = dbg != nullptr;
+	const int CM = mb_post_sm_class(C);      // == C unless the width is forced
+	L.kern = mb_post_sm_kernel(mega, dump, CM);
+	if (!L.kern)
+		return mb_fail(ctx, MB200_EINVAL, "k_posterior_sm has no instantiation for size class %d", CM);
+	// floats of the emission table in shared memory (plain mode: {match, ins} pairs, see k_posterior_sm)
+	const int tsize = mega ? (int) ctx->mega_tsize : 2*ctx->hmm.K*ctx->hmm.KS;
+	L.smem = sizeof(PostSmemHdr) + (size_t)((tsize + 3) & ~3)*sizeof(float)
+	  + (size_t) MB_WARPS_PER_BLOCK*(mega ? MB_SM_ARRAYS_MEGA : MB_SM_ARRAYS)*CM*32*sizeof(float);
+	CU(cudaFuncSetAttribute(L.kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) L.smem));
+	if (ctx->occ_cache_k != tsize*2 + (mega ? 1 : 0))
+		{
+		memset(ctx->occ_cache, 0, sizeof ctx->occ_cache);
+		ctx->occ_cache_k = tsize*2 + (mega ? 1 : 0);
+		}
+	int occ = 0;
+	if (dump)          // another instantiation: not cached
+		CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, L.kern, 32*MB_WARPS_PER_BLOCK, L.smem));
+	else
+		{
+		if (ctx->occ_cache[C] == 0)
+			{
+			CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, L.kern, 32*MB_WARPS_PER_BLOCK, L.smem));
+			ctx->occ_cache[C] = occ;
+			}
+		occ = ctx->occ_cache[C];
+		}
+	if (occ <= 0)
+		return mb_fail(ctx, MB200_ECUDA, "k_posterior_sm (CM=%d) cannot be resident (smem %zu)", CM, L.smem);
+	const uint32_t need_blocks = (pc.nchains + MB_WARPS_PER_BLOCK - 1)/MB_WARPS_PER_BLOCK;
+	const uint32_t nblocks = std::max(1u, std::min((uint32_t) occ*ctx->prop.multiProcessorCount, need_blocks));
+	const size_t nwarps = (size_t) nblocks*MB_WARPS_PER_BLOCK;
+	// scratch geometry; shrink the resident warp count if the Forward-M spill would not fit
+	PostParams &P = L.P;
+	memset(&P, 0, sizeof P);
+	P.lxmax = pc.lxmax;
+	// Forward-M spill, R rows of W columns per step: a strip slot of fm_rows steps per strip of a
+	// single pair, or the steps of a chain (at most its Forward steps + 30), which always has one strip
+	const int R = ctx->plan.R;
+	const uint32_t W = 32u*C;
+	const uint32_t nstrips = (pc.lymax + W - 1)/W;
+	P.fm_rows = mb_fwd_steps(pc.lxmax, R) + 31;
+	P.fm_stride = std::max<size_t>((size_t) nstrips*P.fm_rows, pc.fsteps + 31)*R*W;
+	P.edge_stride = 2*((size_t) pc.lxmax + 2);
+	P.rows_stride = (size_t) pc.rows*MB_CAP;
+	P.rowcnt_stride = ((size_t) pc.rows + 31)/16*16;
+	// bytes per warp of the arrays fm, edge, rows, rowcnt and chainbuf
+	const size_t bytes[5] = { P.fm_stride*4, P.edge_stride*16, P.rows_stride*8, P.rowcnt_stride,
+	  (size_t) MB_CHAIN_BUF*4 };
+	const size_t per_warp = bytes[0] + bytes[1] + bytes[2] + bytes[3] + bytes[4];
+	size_t total_b = 0;
+	if (free_b == 0)
+		cudaMemGetInfo(&free_b, &total_b);
+	DevBuf &scratch = ctx->d_post_scratch[C];
+	const size_t held = scratch.cap;
+	const size_t have = free_b + held;
+	size_t use_warps = nwarps;
+	if (per_warp*use_warps > have*8/10)
+		use_warps = std::max<size_t>(MB_WARPS_PER_BLOCK, (have*8/10/per_warp)/MB_WARPS_PER_BLOCK*MB_WARPS_PER_BLOCK);
+	L.nblocks = (uint32_t)(use_warps/MB_WARPS_PER_BLOCK);
+	// one buffer holds the five arrays of all warps, each starting on a 256-byte boundary
+	size_t off[6] = {};
+	for (int a = 0; a < 5; ++a)
+		off[a + 1] = off[a] + (bytes[a]*use_warps + 255)/256*256;
+	ENSURE(scratch, off[5]);
+	if (scratch.cap != held)
+		free_b = 0;                        // it was (re)allocated: ask again for the next size class
+	P.h = ctx->hmm;
+	P.matchT = (const float *)(mega ? ctx->d_megaT.p : ctx->d_matchT.p);
+	P.insT = (const float *)(mega ? ctx->d_insP.p : ctx->d_insT.p);
+	P.mega_nf = ctx->mega_nf; P.mega_tsize = ctx->mega_tsize;
+	memcpy(P.mega_base, ctx->mega_base, sizeof P.mega_base);
+	memcpy(P.mega_alpha, ctx->mega_alpha, sizeof P.mega_alpha);
+	P.codes = (const uint8_t *) ctx->d_codes.p;
+	P.seqoff = (const uint64_t *) ctx->d_seqoff.p;
+	P.seqlen = (const uint32_t *) ctx->d_seqlen.p;
+	P.px = (const uint32_t *) ctx->d_px.p;
+	P.py = (const uint32_t *) ctx->d_py.p;
+	P.order = (const uint32_t *) ctx->d_order.p;
+	P.chain = (const uint32_t *) ctx->d_chain.p + pc.chain0;
+	P.nwork = pc.nchains;
+	P.counter = (uint32_t *)((char *) ctx->d_cursor.p + 16) + C;
+	P.fm = (float *)((char *) scratch.p + off[0]);
+	P.edge = (float4 *)((char *) scratch.p + off[1]);
+	P.rows = (mb200_entry *)((char *) scratch.p + off[2]);
+	P.rowcnt = (uint8_t *)((char *) scratch.p + off[3]);
+	P.chainbuf = (uint32_t *)((char *) scratch.p + off[4]);
+	P.rowoff = (uint32_t *) ctx->d_rowoff.p;
+	P.rowbase = (const uint64_t *) ctx->d_rowbase.p;
+	P.entries = (mb200_entry *) ctx->d_entries.p;
+	P.ent_cap = ent_cap;
+	P.ent_cursor = (unsigned long long *) ctx->d_cursor.p;
+	P.entbase = (uint64_t *) ctx->d_entbase.p;
+	P.nnz = (uint32_t *) ctx->d_nnz.p;
+	P.ea = (float *) ctx->d_ea.p;
+	P.err = (int *)((char *) ctx->d_cursor.p + 8);
+	if (dbg)
+		{
+		P.dbg_fwd = dbg->fwd; P.dbg_bwd = dbg->bwd; P.dbg_post = dbg->post; P.dbg_total = dbg->total;
+		P.dbg_pair = dbg->pair;
+		}
+	P.cmax = (uint32_t) C;
+	return MB200_OK;
+	}
+
+// The posterior stage over the installed pair list (mb_store_set_pairs)
 static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, int force_c)
 	{
 	const uint32_t np = (uint32_t) ctx->h_px.size();
-	if (!ctx->have_hmm || ctx->nseq == 0)
-		return mb_fail(ctx, MB200_EINVAL, "mb200_posteriors: call mb200_set_hmm and mb200_set_seqs first");
 	cudaSetDevice(ctx->device);
 	cudaStream_t st = ctx->stream;
 	CU(cudaEventRecord(ctx->ev0, st));
-	if (!ctx->plan_valid || ctx->plan_force_c != force_c)
+	const PostPlan &plan = ctx->plan;
+	if (!plan.valid || plan.force_c != force_c)
 		{
-		const int rc = prepare_plan(ctx, force_c);
+		const int rc = build_plan(ctx, force_c, ctx->mega ? 1 : MB_PLAIN_ROWS);
 		if (rc != MB200_OK)
 			return rc;
 		}
-	ctx->stats.cells = ctx->plan_cells;
-	uint64_t est_entries = std::max(ctx->plan_est_entries, ctx->last_used_entries);
-	const auto &bins = ctx->plan_bins;
-	const auto &bin_start = ctx->plan_bin_start;
+	// one control block = { entry cursor u64, error flag i32, pad, work cursors u32[MB_MAX_C+1] }:
+	// a single memset per attempt and a single 16-byte read-back
+	const size_t cursor_bytes = 16 + (MB_MAX_C + 1)*sizeof(uint32_t);
+	ENSURE(ctx->d_cursor, cursor_bytes);
+	ctx->stats.cells = plan.cells;
+	uint64_t est_entries = std::max(plan.est_entries, ctx->last_used_entries);
 
 	bool done = false;
 	for (int attempt = 0; attempt < 3; ++attempt)
 		{
 		ENSURE(ctx->d_entries, (est_entries + 64)*sizeof(mb200_entry));
-		CU(cudaMemsetAsync(ctx->d_cursor.p, 0, 16 + (MB_MAX_C + 1)*sizeof(uint32_t), st));
+		CU(cudaMemsetAsync(ctx->d_cursor.p, 0, cursor_bytes, st));
 		CU(cudaEventRecord(ctx->ev1, st));
 		for (int k = 0; k < mb200_ctx::kStreams; ++k)
 			CU(cudaStreamWaitEvent(ctx->aux[k], ctx->ev1, 0));
 		// widest bins first: they hold most of the work, the narrow ones fill the tails
 		int nlaunched = 0;
-		size_t free_b = 0, total_b = 0;
+		size_t free_b = 0;
 		for (int C = MB_MAX_C; C >= 1; --C)
 			{
-			const auto &b = bins[C];
-			if (b.empty())
+			if (plan.cls[C].nchains == 0)
 				continue;
-			cudaStream_t ks = ctx->aux[nlaunched % mb200_ctx::kStreams];
-			++nlaunched;
-			const uint32_t lxmax = ctx->plan_lxmax[C], lymax = ctx->plan_lymax[C];
-			const uint32_t W = 32u*C;
-			const uint32_t nstrips = (lymax + W - 1)/W;
-			int occ = 0;
-			const bool mega = ctx->mega;
-			const bool dump = dbg != nullptr;
-			const int CM = mb_post_sm_class(C);      // == C unless the width is forced
-			const void *kern = mb_post_sm_kernel(mega, dump, CM);
-			if (!kern)
-				return mb_fail(ctx, MB200_EINVAL, "k_posterior_sm has no instantiation for size class %d", CM);
-			// floats of the emission table in shared memory (plain mode: {match, ins} pairs, see k_posterior_sm)
-			const int tsize = mega ? (int) ctx->mega_tsize : 2*ctx->hmm.K*ctx->hmm.KS;
-			const size_t smem = sizeof(PostSmemHdr) + (size_t)((tsize + 3) & ~3)*sizeof(float)
-			  + (size_t) MB_WARPS_PER_BLOCK*(mega ? MB_SM_ARRAYS_MEGA : MB_SM_ARRAYS)*CM*32*sizeof(float);
-			CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
-			if (ctx->occ_cache_k != tsize*2 + (mega ? 1 : 0))
-				{
-				memset(ctx->occ_cache, 0, sizeof ctx->occ_cache);
-				ctx->occ_cache_k = tsize*2 + (mega ? 1 : 0);
-				}
-			if (dump)          // another instantiation: not cached
-				CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 32*MB_WARPS_PER_BLOCK, smem));
-			else
-				{
-				if (ctx->occ_cache[C] == 0)
-					{
-					CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, 32*MB_WARPS_PER_BLOCK, smem));
-					ctx->occ_cache[C] = occ;
-					}
-				occ = ctx->occ_cache[C];
-				}
-			if (occ <= 0)
-				return mb_fail(ctx, MB200_ECUDA, "k_posterior_sm (CM=%d) cannot be resident (smem %zu)", CM, smem);
-			uint32_t nblocks = (uint32_t) occ*ctx->prop.multiProcessorCount;
-			const uint32_t nchains = bin_start[C + 1] - bin_start[C];
-			const uint32_t need_blocks = (nchains + MB_WARPS_PER_BLOCK - 1)/MB_WARPS_PER_BLOCK;
-			nblocks = std::max(1u, std::min(nblocks, need_blocks));
-			const size_t nwarps = (size_t) nblocks*MB_WARPS_PER_BLOCK;
-			// scratch geometry; shrink the resident warp count if the Forward-M spill would not fit
-			PostParams P;
-			memset(&P, 0, sizeof P);
-			P.lxmax = lxmax;
-			// Forward-M spill, R rows of W columns per step: a strip slot of fm_rows steps per strip of a
-			// single pair, or the steps of a chain (at most its Forward steps + 30), which always has one strip
-			const int R = mega ? 1 : MB_PLAIN_ROWS;
-			P.fm_rows = mb_fwd_steps(lxmax, R) + 31;
-			P.fm_stride = std::max<size_t>((size_t) nstrips*P.fm_rows,
-			  (R == 1 ? ctx->plan_fmax[C] : ctx->plan_fsteps[C]) + 31)*R*W;
-			P.edge_stride = 2*((size_t) lxmax + 2);
-			P.rows_stride = (size_t) ctx->plan_rmax[C]*MB_CAP;
-			P.rowcnt_stride = ((size_t) ctx->plan_rmax[C] + 31)/16*16;
-			// bytes per warp of the arrays fm, edge, rows, rowcnt and chainbuf
-			const size_t bytes[5] = { P.fm_stride*4, P.edge_stride*16, P.rows_stride*8, P.rowcnt_stride,
-			  (size_t) MB_CHAIN_BUF*4 };
-			const size_t per_warp = bytes[0] + bytes[1] + bytes[2] + bytes[3] + bytes[4];
-			if (free_b == 0)
-				cudaMemGetInfo(&free_b, &total_b);
-			DevBuf &scratch = ctx->d_post_scratch[C];
-			const size_t held = scratch.cap;
-			const size_t have = free_b + held;
-			size_t use_warps = nwarps;
-			if (per_warp*use_warps > have*8/10)
-				use_warps = std::max<size_t>(MB_WARPS_PER_BLOCK, (have*8/10/per_warp)/MB_WARPS_PER_BLOCK*MB_WARPS_PER_BLOCK);
-			nblocks = (uint32_t)(use_warps/MB_WARPS_PER_BLOCK);
-			// one buffer holds the five arrays of all warps, each starting on a 256-byte boundary
-			size_t off[6] = {};
-			for (int a = 0; a < 5; ++a)
-				off[a + 1] = off[a] + (bytes[a]*use_warps + 255)/256*256;
-			ENSURE(scratch, off[5]);
-			if (scratch.cap != held)
-				free_b = 0;                        // it was (re)allocated: ask again for the next size class
-			P.h = ctx->hmm;
-			P.matchT = (const float *)(mega ? ctx->d_megaT.p : ctx->d_matchT.p);
-			P.insT = (const float *)(mega ? ctx->d_insP.p : ctx->d_insT.p);
-			P.mega_nf = ctx->mega_nf; P.mega_tsize = ctx->mega_tsize;
-			memcpy(P.mega_base, ctx->mega_base, sizeof P.mega_base);
-			memcpy(P.mega_alpha, ctx->mega_alpha, sizeof P.mega_alpha);
-			P.codes = (const uint8_t *) ctx->d_codes.p;
-			P.seqoff = (const uint64_t *) ctx->d_seqoff.p;
-			P.seqlen = (const uint32_t *) ctx->d_seqlen.p;
-			P.px = (const uint32_t *) ctx->d_px.p;
-			P.py = (const uint32_t *) ctx->d_py.p;
-			P.order = (const uint32_t *) ctx->d_order.p;
-			P.chain = (const uint32_t *) ctx->d_chain.p + bin_start[C];
-			P.nwork = nchains;
-			P.counter = (uint32_t *)((char *) ctx->d_cursor.p + 16) + C;
-			P.fm = (float *)((char *) scratch.p + off[0]);
-			P.edge = (float4 *)((char *) scratch.p + off[1]);
-			P.rows = (mb200_entry *)((char *) scratch.p + off[2]);
-			P.rowcnt = (uint8_t *)((char *) scratch.p + off[3]);
-			P.chainbuf = (uint32_t *)((char *) scratch.p + off[4]);
-			P.rowoff = (uint32_t *) ctx->d_rowoff.p;
-			P.rowbase = (const uint64_t *) ctx->d_rowbase.p;
-			P.entries = (mb200_entry *) ctx->d_entries.p;
-			P.ent_cap = est_entries;
-			P.ent_cursor = (unsigned long long *) ctx->d_cursor.p;
-			P.entbase = (uint64_t *) ctx->d_entbase.p;
-			P.nnz = (uint32_t *) ctx->d_nnz.p;
-			P.ea = (float *) ctx->d_ea.p;
-			P.err = (int *)((char *) ctx->d_cursor.p + 8);
-			if (dbg)
-				{
-				P.dbg_fwd = dbg->fwd; P.dbg_bwd = dbg->bwd; P.dbg_post = dbg->post; P.dbg_total = dbg->total;
-				P.dbg_pair = dbg->pair;
-				}
-			P.cmax = (uint32_t) C;
-			void *args[] = { &P };
-			CU(cudaLaunchKernel(kern, dim3(nblocks), dim3(32*MB_WARPS_PER_BLOCK), args, smem, ks));
+			ClassLaunch L;
+			const int rc = class_launch(ctx, C, dbg, est_entries, free_b, L);
+			if (rc != MB200_OK)
+				return rc;
+			void *args[] = { &L.P };
+			CU(cudaLaunchKernel(L.kern, dim3(L.nblocks), dim3(32*MB_WARPS_PER_BLOCK), args, L.smem,
+			  ctx->aux[nlaunched++ % mb200_ctx::kStreams]));
 			ctx->stats.kernel_launches++;
 			}
 		for (int k = 0; k < mb200_ctx::kStreams; ++k)
@@ -700,12 +675,13 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 	return MB200_OK;
 	}
 
-// a pair list given by the caller: the store no longer holds it, and the plan is rebuilt for it
-static void install_pairs(mb200_ctx *ctx, uint32_t npairs, const uint32_t *pair_x, const uint32_t *pair_y)
+// the new pair list of a posterior call, once there are tables and sequences
+static int install_pairs(mb200_ctx *ctx, StorePairs pairs, uint32_t lo, uint32_t hi, const uint32_t *px, const uint32_t *py)
 	{
-	ctx->h_px.assign(pair_x, pair_x + npairs);
-	ctx->h_py.assign(pair_y, pair_y + npairs);
-	mb_store_set_pairs(ctx, PAIRS_LIST);
+	if (!ctx->have_hmm || ctx->nseq == 0)
+		return mb_fail(ctx, MB200_EINVAL, "mb200_posteriors: call mb200_set_hmm and mb200_set_seqs first");
+	cudaSetDevice(ctx->device);
+	return mb_store_set_pairs(ctx, pairs, lo, hi, px, py);
 	}
 
 int mb200_posteriors(mb200_ctx *ctx, uint32_t npairs, const uint32_t *pair_x, const uint32_t *pair_y,
@@ -713,42 +689,14 @@ int mb200_posteriors(mb200_ctx *ctx, uint32_t npairs, const uint32_t *pair_x, co
 	{
 	if (!ctx || npairs == 0 || !pair_x || !pair_y)
 		return mb_fail(ctx, MB200_EINVAL, "mb200_posteriors: bad argument");
-	install_pairs(ctx, npairs, pair_x, pair_y);
+	const int rc = install_pairs(ctx, PAIRS_LIST, 0, npairs, pair_x, pair_y);
+	if (rc != MB200_OK)
+		return rc;
 	const int force_c = (int)((flags >> 8) & 0xff);
 	if (force_c > MB_MAX_C)
 		return mb_fail(ctx, MB200_EINVAL, "forced C %d > %d", force_c, MB_MAX_C);
 	return run_posteriors(ctx, ea_out, nullptr, force_c);
 	}
-
-} // extern "C"
-
-void mb_allpairs_list(uint32_t n, uint32_t p_lo, uint32_t p_hi, std::vector<uint32_t> &px, std::vector<uint32_t> &py)
-	{
-	px.clear();
-	py.clear();
-	uint32_t p = 0;
-	for (uint32_t i = 0; i < n; ++i)
-		{
-		const uint32_t rowlen = n - 1 - i;
-		if (p + rowlen <= p_lo)
-			{
-			p += rowlen;
-			continue;
-			}
-		for (uint32_t j = i + 1; j < n; ++j, ++p)
-			{
-			if (p >= p_hi)
-				return;
-			if (p >= p_lo)
-				{
-				px.push_back(i);
-				py.push_back(j);
-				}
-			}
-		}
-	}
-
-extern "C" {
 
 int mb200_posteriors_allpairs(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi, float *ea_out)
 	{
@@ -759,11 +707,10 @@ int mb200_posteriors_allpairs(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi, floa
 		return mb_fail(ctx, MB200_EINVAL, "pair range [%u,%u) invalid for %llu pairs", p_lo, p_hi,
 		  (unsigned long long) npairs);
 	const StoreState &s = ctx->store;
-	if (!(ctx->plan_valid && s.pairs == PAIRS_RANGE && s.p_lo == p_lo && s.p_hi == p_hi))
-		{
-		mb_allpairs_list(ctx->nseq, p_lo, p_hi, ctx->h_px, ctx->h_py);
-		mb_store_set_pairs(ctx, PAIRS_RANGE, p_lo, p_hi);
-		}
+	int rc = MB200_OK;
+	if (!(ctx->plan.valid && s.pairs == PAIRS_RANGE && s.p_lo == p_lo && s.p_hi == p_hi)
+	  && (rc = install_pairs(ctx, PAIRS_RANGE, p_lo, p_hi, nullptr, nullptr)) != MB200_OK)
+		return rc;
 	mb_store_drop(ctx);
 	return run_posteriors(ctx, ea_out, nullptr, 0);
 	}
@@ -779,8 +726,9 @@ int mb200_calc_post_dense_pair(mb200_ctx *ctx, uint32_t npairs, const uint32_t *
 	ENSURE(ctx->d_dbg, (3*n + 4)*sizeof(float));
 	float *base = (float *) ctx->d_dbg.p;
 	PostDebug dbg = { base, base + n, base + 2*n, base + 3*n, which };
-	install_pairs(ctx, npairs, pair_x, pair_y);
-	const int rc = run_posteriors(ctx, nullptr, &dbg, ctx->debug_force_c);
+	int rc = install_pairs(ctx, PAIRS_LIST, 0, npairs, pair_x, pair_y);
+	if (rc == MB200_OK)
+		rc = run_posteriors(ctx, nullptr, &dbg, ctx->debug_force_c);
 	if (rc != MB200_OK)
 		return rc;
 	CU(cudaMemcpy(post_out, dbg.post, n*sizeof(float), cudaMemcpyDeviceToHost));
@@ -805,10 +753,11 @@ int mb200_debug_plan(mb200_ctx *ctx, uint32_t *npairs, uint32_t *nchains, uint32
 	{
 	if (!ctx || !npairs || !nchains)
 		return mb_fail(ctx, MB200_EINVAL, "mb200_debug_plan: bad argument");
-	if (!ctx->plan_valid)
+	const PostPlan &plan = ctx->plan;
+	if (!plan.valid)
 		return mb_fail(ctx, MB200_EINVAL, "mb200_debug_plan: no plan (run a posterior stage first)");
 	cudaSetDevice(ctx->device);
-	const uint32_t np = (uint32_t) ctx->h_px.size(), nc = ctx->plan_bin_start[MB_MAX_C + 1];
+	const uint32_t np = (uint32_t) ctx->h_px.size(), nc = plan.cls[MB_MAX_C].chain0 + plan.cls[MB_MAX_C].nchains;
 	*npairs = np;
 	*nchains = nc;
 	if (order)
@@ -816,7 +765,11 @@ int mb200_debug_plan(mb200_ctx *ctx, uint32_t *npairs, uint32_t *nchains, uint32
 	if (chain)
 		CU(cudaMemcpy(chain, ctx->d_chain.p, (nc + 1)*sizeof(uint32_t), cudaMemcpyDeviceToHost));
 	if (bin_start)
-		memcpy(bin_start, ctx->plan_bin_start.data(), (MB_MAX_C + 2)*sizeof(uint32_t));
+		{
+		for (int C = 0; C <= MB_MAX_C; ++C)
+			bin_start[C] = plan.cls[C].chain0;          // first chain of size class C (class 0 is never used: 0)
+		bin_start[MB_MAX_C + 1] = nc;
+		}
 	if (limits)
 		{
 		limits[0] = (uint32_t) kChainRows;

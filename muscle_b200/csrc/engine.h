@@ -32,6 +32,23 @@ struct StoreState
 // and their EA vector was computed here; the host index
 constexpr unsigned NEED_ALLPAIRS = 4, NEED_EA = 8, NEED_INDEX = 16;
 
+// Launch plan of the posterior stage: everything that depends only on the pair list, the forced width and
+// R, the rows per lane per step of the emission mode (engine.cu build_plan; mb_store_set_pairs drops it)
+struct PostClass                          // one size class
+	{
+	uint32_t chain0 = 0, nchains = 0;     // its chains: [chain0, chain0 + nchains) of d_chain
+	uint32_t lxmax = 0, lymax = 0;
+	uint64_t fsteps = 0;                  // most Forward steps of one chain, at R rows per step
+	uint64_t rows = 0;                    // most rows of one chain (sum of LX)
+	};
+struct PostPlan
+	{
+	bool valid = false;
+	int force_c = 0, R = 1;
+	uint64_t cells = 0, est_entries = 0;
+	PostClass cls[MB_MAX_C + 1];
+	};
+
 struct mb200_ctx
 	{
 	int device = 0;
@@ -68,12 +85,12 @@ struct mb200_ctx
 	std::vector<uint32_t> h_nnz;
 	std::vector<uint64_t> h_entbase;
 	DevBuf d_px, d_py, d_order, d_chain;    // d_order: pairs chain after chain; d_chain: offsets of the chains in it
-	DevBuf d_rowoff, d_rowbase, d_entries, d_cursor, d_entbase, d_nnz, d_ea;     // d_cursor: control block, see prepare_plan
+	DevBuf d_rowoff, d_rowbase, d_entries, d_cursor, d_entbase, d_nnz, d_ea;     // d_cursor: control block, see run_posteriors
 	DevBuf d_entries2;                // second value buffer for the Jacobi update
 	DevBuf d_pack_off, d_pack_ent;    // packed image for exchange/export
 	uint64_t xchg_n_offsets = 0, xchg_n_entries = 0;      // sizes announced by mb200_store_exchange_begin
 	// transposed orientation of every pair (rows = positions of Y) for the relax kernel
-	DevBuf d_tr_rowoff, d_tr_rowbase, d_tr_entries, d_tr_entbase, d_tr_perm;
+	DevBuf d_tr_rowoff, d_tr_rowbase, d_tr_entries, d_tr_perm;
 	// column bit masks of every sparse row, both orientations (relax.cu): hdr = {first word slot,
 	// w0 | nw << 16} per row, words = {mask of columns 32w..32w+31, index of the first such entry}
 	DevBuf d_mk_hdr, d_mk_words, d_tr_mk_hdr, d_tr_mk_words;
@@ -89,14 +106,8 @@ struct mb200_ctx
 	bool msa_valid = false;
 	uint32_t *h_pinned = nullptr;     // 64 words of pinned host memory for small read-backs
 
-	// cached launch plan of the posterior stage (depends only on the pair list; mb_store_set_pairs drops it)
-	bool plan_valid = false;
-	int plan_force_c = 0;
-	uint64_t plan_cells = 0, plan_est_entries = 0, last_used_entries = 0;
-	std::vector<std::vector<uint32_t>> plan_bins;                 // pairs per size class
-	std::vector<uint32_t> plan_bin_start, plan_lxmax, plan_lymax;  // bin_start: first chain of each size class
-	std::vector<uint64_t> plan_fmax, plan_rmax;                    // largest chain: Forward rows (sum of LX+2), rows (sum of LX)
-	std::vector<uint64_t> plan_fsteps;                             // largest chain: Forward steps at MB_PLAIN_ROWS rows per step
+	PostPlan plan;
+	uint64_t last_used_entries = 0;
 
 	// per-warp scratch of the posterior kernel, one buffer per bin (PostParams fm, edge, rows, rowcnt, chainbuf)
 	DevBuf d_post_scratch[MB_MAX_C + 1];
@@ -116,7 +127,8 @@ int mb_fail(mb200_ctx *ctx, int code, const char *fmt, ...);
 	  "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } while (0)
 #define ENSURE(buf, bytes) do { if ((buf).ensure(bytes) != 0) \
 	return mb_fail(ctx, MB200_ENOMEM, "device allocation of %zu bytes failed (%s)", (size_t)(bytes), #buf); } while (0)
-void mb_store_set_pairs(mb200_ctx *ctx, StorePairs pairs, uint32_t p_lo = 0, uint32_t p_hi = 0);
+int mb_store_set_pairs(mb200_ctx *ctx, StorePairs pairs, uint32_t lo = 0, uint32_t hi = 0,
+  const uint32_t *px = nullptr, const uint32_t *py = nullptr);
 void mb_store_drop(mb200_ctx *ctx);
 void mb_store_fresh(mb200_ctx *ctx, bool adopted);
 void mb_store_values_written(mb200_ctx *ctx);
@@ -124,4 +136,3 @@ int mb_store_require(mb200_ctx *ctx, const char *who, unsigned needs);
 void mb_store_entry_range(const mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi, uint64_t *e_lo, uint64_t *e_hi);
 int mb_build_masks(mb200_ctx *ctx);             // relax.cu
 void mb_release_post_scratch(mb200_ctx *ctx);
-void mb_allpairs_list(uint32_t n, uint32_t p_lo, uint32_t p_hi, std::vector<uint32_t> &px, std::vector<uint32_t> &py);

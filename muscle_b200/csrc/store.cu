@@ -10,6 +10,7 @@
 #include <cub/cub.cuh>
 #include <algorithm>
 #include <cstring>
+#include <numeric>
 
 // ---------------------------------------------------------------------------------------------
 // one warp per pair: copy the pair's entries to their packed position
@@ -161,11 +162,66 @@ static bool holds_allpairs(const mb200_ctx *ctx)
 	return s.pairs == PAIRS_RANGE && s.p_lo == 0 && s.p_hi == (uint64_t) ctx->nseq*(ctx->nseq - 1)/2;
 	}
 
-// h_px/h_py now hold another pair list (or none): the store and the posterior plan of the old one go
-void mb_store_set_pairs(mb200_ctx *ctx, StorePairs pairs, uint32_t p_lo, uint32_t p_hi)
+// pairs [p_lo,p_hi) of the row-major all-pairs order of n sequences, appended to px/py
+static void allpairs_list(uint32_t n, uint32_t p_lo, uint32_t p_hi, std::vector<uint32_t> &px, std::vector<uint32_t> &py)
 	{
-	ctx->store = StoreState{pairs, p_lo, p_hi};
-	ctx->plan_valid = false;
+	uint32_t p = 0;
+	for (uint32_t i = 0; i < n && p < p_hi; ++i)
+		for (uint32_t j = i + 1; j < n && p < p_hi; ++j, ++p)
+			if (p >= p_lo)
+				{
+				px.push_back(i);
+				py.push_back(j);
+				}
+	}
+
+// first offset slot of every pair of the list and one past the last: LX+1 slots per pair
+static std::vector<uint64_t> row_bases(const mb200_ctx *ctx, const std::vector<uint32_t> &px)
+	{
+	std::vector<uint64_t> rowbase(px.size() + 1, 0);
+	for (size_t k = 0; k < px.size(); ++k)
+		rowbase[k + 1] = rowbase[k] + ctx->h_len[px[k]] + 1;
+	return rowbase;
+	}
+
+// Installs a new pair list: none, pairs [0,hi) of the caller's px/py (PAIRS_LIST, lo = 0), or the all-pairs
+// range [lo,hi).  The store and the posterior plan of the old list go; the per-pair buffers of the store
+// are sized and the list and its row bases uploaded.  A refused list leaves PAIRS_NONE.
+int mb_store_set_pairs(mb200_ctx *ctx, StorePairs pairs, uint32_t lo, uint32_t hi, const uint32_t *px, const uint32_t *py)
+	{
+	ctx->store = StoreState{};
+	ctx->plan.valid = false;
+	ctx->h_px.clear();
+	ctx->h_py.clear();
+	ctx->h_rowbase.clear();
+	if (pairs == PAIRS_NONE)
+		return MB200_OK;
+	if (pairs == PAIRS_LIST)
+		{
+		for (uint32_t k = 0; k < hi; ++k)
+			if (px[k] >= ctx->nseq || py[k] >= ctx->nseq)
+				return mb_fail(ctx, MB200_EINVAL, "pair %u references sequence out of range", k);
+		ctx->h_px.assign(px, px + hi);
+		ctx->h_py.assign(py, py + hi);
+		}
+	else
+		allpairs_list(ctx->nseq, lo, hi, ctx->h_px, ctx->h_py);
+	const uint32_t np = (uint32_t) ctx->h_px.size();
+	ctx->h_rowbase = row_bases(ctx, ctx->h_px);
+	ENSURE(ctx->d_px, np*sizeof(uint32_t));
+	ENSURE(ctx->d_py, np*sizeof(uint32_t));
+	ENSURE(ctx->d_rowbase, (np + 1)*sizeof(uint64_t));
+	ENSURE(ctx->d_rowoff, ctx->h_rowbase[np]*sizeof(uint32_t));
+	ENSURE(ctx->d_entbase, (np + 1)*sizeof(uint64_t));
+	ENSURE(ctx->d_nnz, np*sizeof(uint32_t));
+	ENSURE(ctx->d_ea, np*sizeof(float));
+	cudaStream_t st = ctx->stream;
+	CU(cudaMemcpyAsync(ctx->d_px.p, ctx->h_px.data(), np*sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+	CU(cudaMemcpyAsync(ctx->d_py.p, ctx->h_py.data(), np*sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+	CU(cudaMemcpyAsync(ctx->d_rowbase.p, ctx->h_rowbase.data(), (np + 1)*sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+	ctx->stats.h2d_bytes += 2ull*np*sizeof(uint32_t) + (np + 1)*sizeof(uint64_t);
+	ctx->store = StoreState{pairs, lo, hi};
+	return MB200_OK;
 	}
 
 // the inputs changed, or a posterior stage starts: the pair list and its plan stay
@@ -369,9 +425,9 @@ int mb200_store_exchange_begin(mb200_ctx *ctx, uint64_t n_offsets, uint64_t n_en
 	if (!ctx || !d_offsets || !d_entries || ctx->nseq < 2)
 		return mb_fail(ctx, MB200_EINVAL, "mb200_store_exchange_begin: bad argument");
 	cudaSetDevice(ctx->device);
-	uint64_t rows = 0;
-	for (uint32_t i = 0; i + 1 < ctx->nseq; ++i)
-		rows += (uint64_t)(ctx->h_len[i] + 1)*(ctx->nseq - 1 - i);
+	std::vector<uint32_t> px, py;
+	allpairs_list(ctx->nseq, 0, (uint32_t)((uint64_t) ctx->nseq*(ctx->nseq - 1)/2), px, py);
+	const uint64_t rows = row_bases(ctx, px).back();
 	if (rows != n_offsets)
 		return mb_fail(ctx, MB200_EINVAL, "offset image has %llu slots, all pairs need %llu",
 		  (unsigned long long) n_offsets, (unsigned long long) rows);
@@ -388,28 +444,21 @@ int mb200_store_exchange_begin(mb200_ctx *ctx, uint64_t n_offsets, uint64_t n_en
 // adopt d_pack_off / d_pack_ent (filled by the caller) as the store of all-pairs range [p_lo,p_hi)
 static int adopt_image(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi, uint64_t n_offsets, uint64_t n_entries)
 	{
+	// the image becomes the store's buffers and its pair list is installed before the checks: a refused image
+	// leaves no store, like a failed posterior call, and d_rowoff needs no second buffer of the image's size
+	std::swap(ctx->d_rowoff, ctx->d_pack_off);
+	std::swap(ctx->d_entries, ctx->d_pack_ent);
+	int rc = mb_store_set_pairs(ctx, PAIRS_RANGE, p_lo, p_hi);
+	if (rc != MB200_OK)
+		return rc;
 	cudaStream_t st = ctx->stream;
-	std::vector<uint32_t> px, py;
-	mb_allpairs_list(ctx->nseq, p_lo, p_hi, px, py);
-	const uint32_t np = (uint32_t) px.size();
-	std::vector<uint64_t> rowbase(np + 1, 0);
-	for (uint32_t k = 0; k < np; ++k)
-		rowbase[k + 1] = rowbase[k] + ctx->h_len[px[k]] + 1;
-	if (rowbase[np] != n_offsets)
+	const uint32_t np = (uint32_t) ctx->h_px.size();
+	if (ctx->h_rowbase[np] != n_offsets)
 		return mb_fail(ctx, MB200_EINVAL, "offset image has %llu slots, pair range needs %llu",
-		  (unsigned long long) n_offsets, (unsigned long long) rowbase[np]);
-	ENSURE(ctx->d_px, np*sizeof(uint32_t));
-	ENSURE(ctx->d_py, np*sizeof(uint32_t));
-	ENSURE(ctx->d_rowbase, (np + 1)*sizeof(uint64_t));
-	ENSURE(ctx->d_entbase, (np + 1)*sizeof(uint64_t));
-	ENSURE(ctx->d_nnz, np*sizeof(uint32_t));
-	ENSURE(ctx->d_ea, np*sizeof(float));
+		  (unsigned long long) n_offsets, (unsigned long long) ctx->h_rowbase[np]);
 	ENSURE(ctx->d_tmp, (np + 1)*sizeof(uint64_t));
-	CU(cudaMemcpyAsync(ctx->d_px.p, px.data(), np*sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(ctx->d_py.p, py.data(), np*sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-	CU(cudaMemcpyAsync(ctx->d_rowbase.p, rowbase.data(), (np + 1)*sizeof(uint64_t), cudaMemcpyHostToDevice, st));
 	k_nnz_from_rowoff<<<(np + 255)/256, 256, 0, st>>>(np, (const uint64_t *) ctx->d_rowbase.p,
-	  (const uint32_t *) ctx->d_pack_off.p, (uint32_t *) ctx->d_nnz.p, (uint64_t *) ctx->d_tmp.p);
+	  (const uint32_t *) ctx->d_rowoff.p, (uint32_t *) ctx->d_nnz.p, (uint64_t *) ctx->d_tmp.p);
 	CU(cudaGetLastError());
 	size_t tb = 0;
 	cub::DeviceScan::ExclusiveSum(nullptr, tb, (uint64_t *) ctx->d_tmp.p, (uint64_t *) ctx->d_entbase.p, (int) np, st);
@@ -417,27 +466,13 @@ static int adopt_image(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi, uint64_t n_
 	cub::DeviceScan::ExclusiveSum(ctx->d_tmp2.p, tb, (uint64_t *) ctx->d_tmp.p, (uint64_t *) ctx->d_entbase.p, (int) np, st);
 	CU(cudaGetLastError());
 	ctx->stats.kernel_launches += 2;
-	std::vector<uint32_t> h_nnz(np);
-	std::vector<uint64_t> h_entbase(np);
-	CU(cudaMemcpyAsync(h_nnz.data(), ctx->d_nnz.p, np*sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-	CU(cudaMemcpyAsync(h_entbase.data(), ctx->d_entbase.p, np*sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-	CU(cudaStreamSynchronize(st));
-	uint64_t tot = 0;
-	for (uint32_t k = 0; k < np; ++k)
-		tot += h_nnz[k];
+	if ((rc = read_index(ctx, true)) != MB200_OK)
+		return rc;
+	const uint64_t tot = std::accumulate(ctx->h_nnz.begin(), ctx->h_nnz.end(), (uint64_t) 0);
 	if (tot != n_entries)
 		return mb_fail(ctx, MB200_EINVAL, "entry image has %llu entries, offsets say %llu",
 		  (unsigned long long) n_entries, (unsigned long long) tot);
-	// everything validated: mutate the context
-	std::swap(ctx->d_rowoff, ctx->d_pack_off);
-	std::swap(ctx->d_entries, ctx->d_pack_ent);
-	ctx->h_px.swap(px);
-	ctx->h_py.swap(py);
-	ctx->h_rowbase.swap(rowbase);
-	ctx->h_nnz.swap(h_nnz);
-	ctx->h_entbase.swap(h_entbase);
 	ctx->store_nnz = tot;
-	mb_store_set_pairs(ctx, PAIRS_RANGE, p_lo, p_hi);
 	mb_store_fresh(ctx, true);
 	return MB200_OK;
 	}

@@ -2,7 +2,7 @@
 
 Every case checks, for every pair, the sparse store (row offsets and entry bytes) and the EA against
 the CPU oracle (or the Mega goldens) with tolerance 0, and checks that the library's plan is the one
-the chain rule of prepare_plan (muscle_b200/csrc/engine.cu) gives, chain for chain, so that the cases
+the chain rule of build_plan (muscle_b200/csrc/engine.cu) gives, chain for chain, so that the cases
 keep reaching the boundaries they were built for.  The boundaries are taken from the limits the
 library reports, not hard-coded.  X sequences are windows of a homolog of Y, so that even short
 pairs keep posterior entries >= 0.01 and a wrong kernel cannot pass on empty results.
@@ -26,7 +26,7 @@ def _size_class(c):
 
 
 def mirror_plan(lens, px, py, force_c, max_rows, max_pairs):
-	"""-> (order, chain, bin_start) as prepare_plan builds them: pairs are binned by columns per lane;
+	"""-> (order, chain, bin_start) as build_plan builds them: pairs are binned by columns per lane;
 	inside a bin, pairs with the same Y join the open chain of that Y in store order unless it would
 	pass max_rows Forward rows (sum of LX+2) or max_pairs pairs, or the pair needs more than one strip;
 	chains are ordered by cells, most first, ties in creation order"""

@@ -13,6 +13,7 @@ in one place, which calls a context accepts after each call that produces or dro
   set_seqs                               no store, no MSAs until msa_reset
   store_load_allpairs / exchange commit  consistency and msa_join; guide_tree() only with an EA argument
   unpacked store                         store_set_values refused until store_pack
+  refused store image                    no store
   failed posterior call                  no store
 
 Where a call produces a store or an alignment, the result is compared bit for bit with a fresh
@@ -146,6 +147,18 @@ def test_lifecycle(cuda, tables):
 	e.consistency_iter()
 	ref.consistency_iter()
 	same_store(e, ref)
+
+	# a refused store image leaves no store: an all-pairs image whose entry count is one short
+	e.posteriors(px, py)
+	po, no, pe, ne = ref.store_pack_ptrs()
+	refused(e.store_load_allpairs, 0, npairs, po, no, pe, ne - 1)
+	refused(e.store_nnz)
+	refused(e.export_all)
+	assert e.posteriors_allpairs().tobytes() == ea_ref.tobytes()
+	r = fresh(tables, seqs)
+	r.posteriors_allpairs()
+	same_store(e, r)
+	r.close()
 
 	# a failed posterior call leaves no store
 	e.set_seqs(["A"*21000, "C"*21000, "ACD"])
