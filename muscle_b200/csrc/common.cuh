@@ -18,7 +18,13 @@
 #define MB_SM_ARRAYS_MEGA 7             // MEGA: float4 state + {letters 0..3, eY} + letters 4..7
 #define MB_CHAIN_MAX 32                 // posterior kernel: pairs in one chain (one per lane when the chain is read)
 #define MB_CHAIN_BUF (MB_CHAIN_MAX*38)  // words of per-warp chain scratch: kept counts [pair][lane], totals [pair], final cells [pair][5]
-#define MB_PLAIN_ROWS 2                 // posterior kernel: rows per lane per step of the plain-mode passes (MEGA: 1)
+
+// rows per lane per step of the posterior kernel's Forward and Backward passes: two in plain mode, one in
+// MEGA mode
+__host__ __device__ constexpr int mb_post_rows(bool mega)
+	{
+	return mega ? 1 : 2;
+	}
 
 // Forward steps one lane spends on a pair of LX rows at R rows per step: rows 0..LX, then one separator
 // step.  At R = 2 a pair of even LX starts with one all-LOG_ZERO row (-1), so that its rows pair up as

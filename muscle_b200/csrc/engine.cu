@@ -598,7 +598,7 @@ static int run_posteriors(mb200_ctx *ctx, float *ea_out, const PostDebug *dbg, i
 	const PostPlan &plan = ctx->plan;
 	if (!plan.valid || plan.force_c != force_c)
 		{
-		const int rc = build_plan(ctx, force_c, ctx->mega ? 1 : MB_PLAIN_ROWS);
+		const int rc = build_plan(ctx, force_c, mb_post_rows(ctx->mega));
 		if (rc != MB200_OK)
 			return rc;
 		}

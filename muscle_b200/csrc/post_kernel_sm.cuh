@@ -89,61 +89,96 @@ __device__ __forceinline__ MbSeq mb_seq(const PostParams &P, uint32_t s)
 	return { (int) P.seqlen[s], P.codes + o, reinterpret_cast<const uint2 *>(P.codes) + o, P.insT + o };
 	}
 
-// position i of X as a row of the DP needs it (class, or letters and insert emission); the padding when
-// !in.  Loaded one step ahead of its use.
-struct MbXRow { int code; uint2 letters; float ins; };
+// MEGA mode: position i of X as a row of the DP needs it (letters and insert emission); zeros when !in.
+// Loaded one step ahead of its use.
+struct MbXRow { uint2 letters; float ins; };
 
-template <bool MEGA>
-__device__ __forceinline__ MbXRow mb_x_row(const MbSeq &X, bool in, int i, int pad)
+__device__ __forceinline__ MbXRow mb_x_row(const MbSeq &X, bool in, int i)
 	{
-	MbXRow r = { pad, make_uint2(0u, 0u), 0.0f };
-	if (MEGA)
-		{
-		r.letters = in ? X.letters[i] : make_uint2(0u, 0u);
-		r.ins = in ? X.ins[i] : 0.0f;
-		}
-	else
-		r.code = in ? (int) X.code[i] : pad;
+	MbXRow r;
+	r.letters = in ? X.letters[i] : make_uint2(0u, 0u);
+	r.ins = in ? X.ins[i] : 0.0f;
 	return r;
 	}
 
-// X's side of the emissions of a row: its insert emission, and its {match, insert} table row merow
-// (plain) or xb of mb_mega_emit for its letters (MEGA)
-struct MbXEmit { float ins; const float2 *merow; uint32_t xb[8]; };
+// MEGA mode: X's side of the emissions of a row: its insert emission, and xb of mb_mega_emit for its letters
+struct MbXEmit { float ins; uint32_t xb[8]; };
 
-template <bool MEGA>
-__device__ __forceinline__ MbXEmit mb_x_emit(const PostParams &P, const float *insT, const float2 *meT, int KS,
-  const MbXRow &x)
+__device__ __forceinline__ MbXEmit mb_x_emit(const PostParams &P, const MbXRow &x)
 	{
 	MbXEmit e;
-	e.ins = MEGA ? x.ins : insT[x.code];
-	e.merow = meT + (MEGA ? 0 : x.code*KS);
-	if (MEGA)
-		{
+	e.ins = x.ins;
 #pragma unroll
-		for (int f = 0; f < 8; ++f)
-			e.xb[f] = P.mega_base[f]
-			  + ((f < 4 ? (x.letters.x >> (8*f)) : (x.letters.y >> (8*(f - 4)))) & 255u)*P.mega_alpha[f];
-		}
+	for (int f = 0; f < 8; ++f)
+		e.xb[f] = P.mega_base[f]
+		  + ((f < 4 ? (x.letters.x >> (8*f)) : (x.letters.y >> (8*(f - 4)))) & 255u)*P.mega_alpha[f];
 	return e;
 	}
 
-// {match emission, insert emission of Y} of a column whose staged Y data is at yp / y2p, in a row with
-// X's side xe
-template <bool MEGA>
+// MEGA mode: {match emission, insert emission of Y} of a column whose staged Y data is at yp / y2p, in a
+// row with X's side xe
 __device__ __forceinline__ float2 mb_col_emit(const float *matchT, const MbXEmit &xe, int nf, const uint2 *yp,
   const uint32_t *y2p)
 	{
-	if (MEGA)
-		{
-		const uint2 y = *yp;
-		return make_float2(mb_mega_emit(matchT, xe.xb, y.x, *y2p, nf), __uint_as_float(y.y));
-		}
-	return xe.merow[*y2p];
+	const uint2 y = *yp;
+	return make_float2(mb_mega_emit(matchT, xe.xb, y.x, *y2p, nf), __uint_as_float(y.y));
 	}
 
-// the five values of a Backward cell (bwdflat3.cpp:95-125)
+// the values of a Forward cell (fwdflat3.cpp:110-140) and s, the LOG_ADD of its five states with their
+// transitions to M, which the cell down-right takes as its diagonal.  diag: s of the cell up-left; uM,
+// uIX, uJX: the cell above; lm: M of the cell to the left, laiy / lajy: its IY / JY plus tII / tJJ
+struct MbFwdCell { float s, m, ix, jx, iy, jy; };
+
+__device__ __forceinline__ MbFwdCell mb_fwd_cell(const MbHmm &h, const LogAdd &la, float diag, float em, float uM,
+  float uIX, float uJX, float laiy, float lajy, float lm, float ex, float eyc)
+	{
+	MbFwdCell r;
+	r.m = ADD(diag, em);
+	r.ix = ADD(la(ADD(uIX, h.tII), ADD(uM, h.tMI)), ex);
+	r.jx = ADD(la(ADD(uJX, h.tJJ), ADD(uM, h.tMJ)), ex);
+	r.iy = ADD(la(laiy, ADD(lm, h.tMI)), eyc);
+	r.jy = ADD(la(lajy, ADD(lm, h.tMJ)), eyc);
+	r.s = la(ADD(r.m, h.tMM), la(ADD(r.ix, h.tIM), la(ADD(r.jx, h.tJM),
+	  la(ADD(r.iy, h.tIM), ADD(r.jy, h.tJM)))));
+	return r;
+	}
+
+// the five values of a Backward cell (bwdflat3.cpp:95-125) from the row below ({M, IX, JX} of this column
+// and M of the next one) and the IY / JY of the cell to the right
 struct MbBwdCell { float m, ix, jx, iy, jy; };
+
+__device__ __forceinline__ MbBwdCell mb_bwd_cell(const MbHmm &h, const LogAdd &la, float mdiag, float vIX, float vJX,
+  float riy, float rjy, float em, float eyc, float ex)
+	{
+	const float nM = ADD(mdiag, em);
+	const float nIX = ADD(vIX, ex);
+	const float nJX = ADD(vJX, ex);
+	const float nIY = ADD(riy, eyc);
+	const float nJY = ADD(rjy, eyc);
+	MbBwdCell r;
+	r.m = la(ADD(h.tMM, nM), la(ADD(h.tMI, nIX), la(ADD(h.tMJ, nJX),
+	  la(ADD(h.tMI, nIY), ADD(h.tMJ, nJY)))));
+	r.ix = la(ADD(h.tII, nIX), ADD(h.tIM, nM));
+	r.jx = la(ADD(h.tJJ, nJX), ADD(h.tJM, nM));
+	r.iy = la(ADD(h.tII, nIY), ADD(h.tIM, nM));
+	r.jy = la(ADD(h.tJJ, nJY), ADD(h.tJM, nM));
+	return r;
+	}
+
+// posterior score of cell (i, col) (calcposteriorflat.cpp:14-22) from its Forward and Backward M; when
+// dump, the cell's Backward M and probability go to the dense dump (row 0 is not a cell of it)
+__device__ __forceinline__ float mb_post_score(const PostParams &P, bool dump, int i, int LY, int col, float fmv,
+  float m, float total)
+	{
+	const float score = __fsub_rn(ADD(fmv, m), total);
+	if (dump && i >= 1)
+		{
+		P.dbg_bwd[(size_t)(i - 1)*LY + col] = m;
+		P.dbg_post[(size_t)(i - 1)*LY + col] =
+		  score < P.h.minScore ? 0.0f : (score >= 0.0f ? 1.0f : mb_expf_glibc(score));
+		}
+	return score;
+	}
 
 // one strip of a chain: j0, the position in Y of its first column; nl, the lanes that hold columns of it;
 // cn, the lane's columns up to LY
@@ -491,8 +526,7 @@ __global__ void __launch_bounds__(32*MB_WARPS_PER_BLOCK, (MEGA || CM > 14) ? 4 :
 k_posterior_sm(const PostParams P)
 	{
 	constexpr int NARR = MEGA ? MB_SM_ARRAYS_MEGA : MB_SM_ARRAYS;
-	constexpr int R = MEGA ? 1 : MB_PLAIN_ROWS;       // rows per lane per step of Forward and Backward
-	static_assert(R == 1 || R == 2, "the passes are written for one row or a pair of rows per step");
+	constexpr int R = mb_post_rows(MEGA);
 	extern __shared__ __align__(16) unsigned char smem_raw[];
 	PostSmemHdr &sm = *reinterpret_cast<PostSmemHdr *>(smem_raw);
 	const MbHmm h = P.h;
@@ -564,34 +598,34 @@ k_posterior_sm(const PostParams P)
 		// Lane l steps through the chain's pairs one after the other: rows 0..LX of a pair, then one
 		// separator step that resets the lane's state records to LOG_ZERO and passes LOG_ZERO on, so
 		// that row 0 of the next pair sees exactly the border of a fresh pair.  Pair k starts at chain
-		// step Fk + l, Fk = sum over earlier pairs of (LX + 2).
-		if constexpr (R == 1)
+		// step Fk + l, Fk = sum over earlier pairs of (LX + 2).  MEGA mode: one row per lane per step.
+		if constexpr (MEGA)
 			for (int strip = 0; strip < g.n; ++strip)
 				{
 				const auto [j0, nl, cn, last] = g.at(strip, lane);
 				const auto [edgeIn, edgeOut] = mb_strip_edges(edge0, edge1, strip);
 				float *fms = fm + (size_t) strip*P.fm_rows*W;
 
-				mb_stage_y<MEGA>(Y, j0 + lane*C, C, lane, h.pad, st, ye, y2);
+				mb_stage_y<true>(Y, j0 + lane*C, C, lane, h.pad, st, ye, y2);
 				float outM = Z, outAIY = Z, outAJY = Z, outS = Z;
 				float dprev = Z;
 				float bIX = Z, bJX = Z;
 				const int nsteps = sumLX + 2*nch - 2 + nl;
 				int kp = 0, r0 = lane;                // the lane's pair and the step of its row 0
 				MbSeq X = mb_seq(P, P.px[cpairs[0]]);
-				MbXRow xPref = mb_x_row<MEGA>(X, false, 0, h.pad);
+				MbXRow xPref = mb_x_row(X, false, 0);
 				for (int t = 0; t < nsteps; ++t)
 					{
 					const int i = t - r0;
 					const MbXRow x = xPref;
-					xPref = mb_x_row<MEGA>(X, i >= 0 && i < X.len, i, h.pad);
+					xPref = mb_x_row(X, i >= 0 && i < X.len, i);
 					float Lm = __shfl_up_sync(MB_FULL, outM, 1);
 					float Laiy = __shfl_up_sync(MB_FULL, outAIY, 1);
 					float Lajy = __shfl_up_sync(MB_FULL, outAJY, 1);
 					float Ls = __shfl_up_sync(MB_FULL, outS, 1);
 					if (i >= 0 && i <= X.len && lane < nl)
 						{
-						const MbXEmit xe = mb_x_emit<MEGA>(P, sm.insT, meT, h.KS, x);
+						const MbXEmit xe = mb_x_emit(P, x);
 						const float ex = xe.ins;
 						if (lane == 0)
 							{
@@ -635,23 +669,18 @@ k_posterior_sm(const PostParams P)
 						for (int c = 0; c < cn; ++c, sp += 32, yp += 32, y2p += 32, dst += 32)
 							{
 							const float4 v = *sp;                      // {S, M, IX, JX} of row i-1
-							const auto [em, eyc] = mb_col_emit<MEGA>(matchT, xe, nf, yp, y2p);
-							const float m = ADD(diag, em);
-							ix = ADD(la(ADD(v.z, h.tII), ADD(v.y, h.tMI)), ex);
-							jx = ADD(la(ADD(v.w, h.tJJ), ADD(v.y, h.tMJ)), ex);
-							iy = ADD(la(laiy, ADD(lm, h.tMI)), eyc);
-							jy = ADD(la(lajy, ADD(lm, h.tMJ)), eyc);
-							const float s = la(ADD(m, h.tMM), la(ADD(ix, h.tIM), la(ADD(jx, h.tJM),
-							  la(ADD(iy, h.tIM), ADD(jy, h.tJM)))));
+							const auto [em, eyc] = mb_col_emit(matchT, xe, nf, yp, y2p);
+							const MbFwdCell f = mb_fwd_cell(h, la, diag, em, v.y, v.z, v.w, laiy, lajy, lm, ex, eyc);
+							ix = f.ix; jx = f.jx; iy = f.iy; jy = f.jy;
 							diag = v.x;
-							*sp = make_float4(s, m, ix, jx);
-							lm = m;
-							laiy = ADD(iy, h.tII);
-							lajy = ADD(jy, h.tJJ);
-							sLast = s;
-							*dst = m;
+							*sp = make_float4(f.s, f.m, f.ix, f.jx);
+							lm = f.m;
+							laiy = ADD(f.iy, h.tII);
+							lajy = ADD(f.jy, h.tJJ);
+							sLast = f.s;
+							*dst = f.m;
 							if (dump)
-								P.dbg_fwd[(size_t)(i - 1)*LY + j0 + lane*C + c] = m;
+								P.dbg_fwd[(size_t)(i - 1)*LY + j0 + lane*C + c] = f.m;
 							}
 						if (last && i == X.len && lane == g.lcl)    // cell (LX,LY) is the lane's last
 							{
@@ -702,7 +731,8 @@ k_posterior_sm(const PostParams P)
 				int pad = ~X.len & 1, nq = X.len/2 + 1;   // row -1 or not; the pair's row steps
 				auto xcode = [&](int i) { return i >= 1 && i <= X.len ? (int) X.code[i - 1] : h.pad; };
 				int xa = h.pad, xb = xcode(1 - pad);     // classes of the next step's rows
-				// the left border of row i in lane 0 of strip 0: the start scores at (0,0), the bIX / bJX chain
+				// the left border of row i in lane 0 of strip 0: the start scores at (0,0), the bIX / bJX chain.
+				// It stays apart from the MEGA pass's: each form tried for both changed one mode's SASS.
 				auto border = [&](int i, float ex, float &Lm, float &Laiy, float &Lajy, float &Ls)
 					{
 					Lm = Z;
@@ -772,33 +802,21 @@ k_posterior_sm(const PostParams P)
 							const uint32_t yc = *y2p;
 							const float2 ea = mea[yc];                 // {match of row a, insert of Y}
 							const float emb = reinterpret_cast<const float *>(meb + yc)[0];
-							const float eyc = ea.y;
-							const float ma = ADD(diaga, ea.x);
-							const float ixa = ADD(la(ADD(v.z, h.tII), ADD(v.y, h.tMI)), exa);
-							const float jxa = ADD(la(ADD(v.w, h.tJJ), ADD(v.y, h.tMJ)), exa);
-							const float iya = ADD(la(laiya, ADD(lma, h.tMI)), eyc);
-							const float jya = ADD(la(lajya, ADD(lma, h.tMJ)), eyc);
-							const float sa = la(ADD(ma, h.tMM), la(ADD(ixa, h.tIM), la(ADD(jxa, h.tJM),
-							  la(ADD(iya, h.tIM), ADD(jya, h.tJM)))));
-							const float mb = ADD(diagb, emb);
-							ixb = ADD(la(ADD(ixa, h.tII), ADD(ma, h.tMI)), exb);
-							jxb = ADD(la(ADD(jxa, h.tJJ), ADD(ma, h.tMJ)), exb);
-							iyb = ADD(la(laiyb, ADD(lmb, h.tMI)), eyc);
-							jyb = ADD(la(lajyb, ADD(lmb, h.tMJ)), eyc);
-							const float sb = la(ADD(mb, h.tMM), la(ADD(ixb, h.tIM), la(ADD(jxb, h.tJM),
-							  la(ADD(iyb, h.tIM), ADD(jyb, h.tJM)))));
+							const MbFwdCell a = mb_fwd_cell(h, la, diaga, ea.x, v.y, v.z, v.w, laiya, lajya, lma, exa, ea.y);
+							const MbFwdCell b = mb_fwd_cell(h, la, diagb, emb, a.m, a.ix, a.jx, laiyb, lajyb, lmb, exb, ea.y);
+							ixb = b.ix; jxb = b.jx; iyb = b.iy; jyb = b.jy;
 							diaga = v.x;
-							diagb = sa;
-							*sp = make_float4(sb, mb, ixb, jxb);
-							lma = ma; laiya = ADD(iya, h.tII); lajya = ADD(jya, h.tJJ); sLasta = sa;
-							lmb = mb; laiyb = ADD(iyb, h.tII); lajyb = ADD(jyb, h.tJJ); sLastb = sb;
-							*dst = make_float2(ma, mb);
+							diagb = a.s;
+							*sp = make_float4(b.s, b.m, b.ix, b.jx);
+							lma = a.m; laiya = ADD(a.iy, h.tII); lajya = ADD(a.jy, h.tJJ); sLasta = a.s;
+							lmb = b.m; laiyb = ADD(b.iy, h.tII); lajyb = ADD(b.jy, h.tJJ); sLastb = b.s;
+							*dst = make_float2(a.m, b.m);
 							if (dump)
 								{
 								if (ia >= 1)
-									P.dbg_fwd[(size_t)(ia - 1)*LY + j0 + lane*C + c] = ma;
+									P.dbg_fwd[(size_t)(ia - 1)*LY + j0 + lane*C + c] = a.m;
 								if (ia >= 0)
-									P.dbg_fwd[(size_t) ia*LY + j0 + lane*C + c] = mb;
+									P.dbg_fwd[(size_t) ia*LY + j0 + lane*C + c] = b.m;
 								}
 							}
 						if (last && ia + 1 == X.len && lane == g.lcl)    // cell (LX,LY): row b, the lane's last
@@ -869,21 +887,22 @@ k_posterior_sm(const PostParams P)
 		const float keepScore = fmaxf(h.minScore, __uint_as_float(0xc0935d8eu));
 		uint32_t kept = 0;
 		bool overflow = false;
-		if constexpr (R == 1)
+		// MEGA mode: one row per lane per step.
+		if constexpr (MEGA)
 			for (int strip = g.n - 1; strip >= 0; --strip)
 				{
 				const auto [j0, nl, cn, last] = g.at(strip, lane);
 				const auto [edgeIn, edgeOut] = mb_strip_edges(edge0, edge1, strip);
 				const float *fms = fm + (size_t) strip*P.fm_rows*W;
 
-				mb_stage_y<MEGA>(Y, j0 + lane*C + 1, C, lane, h.pad, st, ye, y2);
+				mb_stage_y<true>(Y, j0 + lane*C + 1, C, lane, h.pad, st, ye, y2);
 				float outM = Z, outIY = Z, outJY = Z;
 				uint32_t outCnt = 0;
 				float dprev = Z;
 				const int nsteps = sumLX + nch - 2 + nl;
 				int kp = nch - 1, u0 = nl - 1 - lane;   // the lane's pair and the step of its row LX
 				MbSeq X = mb_seq(P, P.px[cpairs[nch - 1]]);
-				MbXRow xPref = mb_x_row<MEGA>(X, false, 0, h.pad);
+				MbXRow xPref = mb_x_row(X, false, 0);
 				int fk = sumLX - X.len + 2*(nch - 1);   // chain Forward step of the pair's row 0, less the lane
 				int rk = sumLX - X.len;               // chain row of the pair's row 1 in rows / rowcnt
 				float total = ctotal[nch - 1];
@@ -891,7 +910,7 @@ k_posterior_sm(const PostParams P)
 					{
 					const int i = X.len - u + u0;
 					const MbXRow x = xPref;
-					xPref = mb_x_row<MEGA>(X, i >= 2 && i <= X.len, i - 1, h.pad);
+					xPref = mb_x_row(X, i >= 2 && i <= X.len, i - 1);
 					float Rm = __shfl_down_sync(MB_FULL, outM, 1);
 					float Riy = __shfl_down_sync(MB_FULL, outIY, 1);
 					float Rjy = __shfl_down_sync(MB_FULL, outJY, 1);
@@ -910,28 +929,16 @@ k_posterior_sm(const PostParams P)
 								Rm = e.x; Riy = e.y; Rjy = e.z; cnt = __float_as_uint(e.w);
 								}
 							}
-						const MbXEmit xe = mb_x_emit<MEGA>(P, sm.insT, meT, h.KS, x);
+						const MbXEmit xe = mb_x_emit(P, x);
 						const float ex = xe.ins;
 						const int t = fk + i + lane;
 						const int col0 = j0 + lane*C;
 						float mdiag = dprev;
 						dprev = Rm;
 						float riy = Riy, rjy = Rjy, mFirst = Z;
-						// posterior score (calcposteriorflat.cpp:14-22) and its threshold; columns arrive descending,
-						// so bit c of hits ends up on column c
+						// the posterior scores' threshold: columns arrive descending, so bit c of hits ends up on column c
 						uint32_t hits = 0;
-						auto post = [&](int c, float fmv, float m)
-							{
-							const float score = __fsub_rn(ADD(fmv, m), total);
-							hits = 2u*hits + (score >= h.minScore ? 1u : 0u);
-							if (DUMP && cpairs[kp] == P.dbg_pair)
-								{
-								P.dbg_bwd[(size_t)(i - 1)*LY + col0 + c] = m;
-								P.dbg_post[(size_t)(i - 1)*LY + col0 + c] =
-								  score < h.minScore ? 0.0f : (score >= 0.0f ? 1.0f : mb_expf_glibc(score));
-								}
-							return score;
-							};
+						const bool dump = DUMP && cpairs[kp] == P.dbg_pair;
 						float4 *sp = st + lane;
 						const uint2 *yp = ye + lane;
 						const uint32_t *y2p = y2 + lane;
@@ -942,7 +949,9 @@ k_posterior_sm(const PostParams P)
 							{
 							// cell (LX,LY), the lane's first: the end scores (bwdflat3.cpp:53-61)
 							mdiag = sp->x;
-							*sp = make_float4(h.tSM, h.tSI, h.tSJ, post(c, *src, h.tSM));
+							const float s = mb_post_score(P, dump, i, LY, col0 + c, *src, h.tSM, total);
+							hits = s >= h.minScore ? 1u : 0u;
+							*sp = make_float4(h.tSM, h.tSI, h.tSJ, s);
 							riy = h.tSI; rjy = h.tSJ; mFirst = h.tSM;
 							--c; sp -= 32; yp -= 32; y2p -= 32; src -= 32;
 							}
@@ -962,22 +971,14 @@ k_posterior_sm(const PostParams P)
 							if (c >= 2)
 								fmNext2 = src[-32];                // column c-2
 							const float4 v = *sp;                      // {M, IX, JX, score} of row i+1
-							const auto [em, eyc] = mb_col_emit<MEGA>(matchT, xe, nf, yp, y2p);
-							const float nM = ADD(mdiag, em);
-							const float nIX = ADD(v.y, ex);
-							const float nJX = ADD(v.z, ex);
-							const float nIY = ADD(riy, eyc);
-							const float nJY = ADD(rjy, eyc);
-							const float m = la(ADD(h.tMM, nM), la(ADD(h.tMI, nIX), la(ADD(h.tMJ, nJX),
-							  la(ADD(h.tMI, nIY), ADD(h.tMJ, nJY)))));
-							const float ix = la(ADD(h.tII, nIX), ADD(h.tIM, nM));
-							const float jx = la(ADD(h.tJJ, nJX), ADD(h.tJM, nM));
-							const float iy = la(ADD(h.tII, nIY), ADD(h.tIM, nM));
-							const float jy = la(ADD(h.tJJ, nJY), ADD(h.tJM, nM));
+							const auto [em, eyc] = mb_col_emit(matchT, xe, nf, yp, y2p);
+							const MbBwdCell b = mb_bwd_cell(h, la, mdiag, v.y, v.z, riy, rjy, em, eyc, ex);
+							const float s = mb_post_score(P, dump, i, LY, col0 + c, fmv, b.m, total);
+							hits = 2u*hits + (s >= h.minScore ? 1u : 0u);
 							mdiag = v.x;
-							*sp = make_float4(m, ix, jx, post(c, fmv, m));
-							riy = iy; rjy = jy;
-							mFirst = m;
+							*sp = make_float4(b.m, b.ix, b.jx, s);
+							riy = b.iy; rjy = b.jy;
+							mFirst = b.m;
 							}
 						// the survivors, highest column first (the row's order): the warp runs this loop as often as
 						// the most survivors in one lane, not once per column in which any lane has one
@@ -1108,38 +1109,10 @@ k_posterior_sm(const PostParams P)
 						float mdiaga = dprev, mdiagb = Rma;
 						dprev = Rmb;
 						float riya = Riya, rjya = Rjya, riyb = Riyb, rjyb = Rjyb, mFirsta = Z, mFirstb = Z;
-						// posterior scores (calcposteriorflat.cpp:14-22) and their threshold; columns arrive descending,
-						// so bit c of hits ends up on row a's column c and bit 16+c on row b's
+						// the posterior scores' threshold: columns arrive descending, so bit c of hits ends up on row a's
+						// column c and bit 16+c on row b's
 						uint32_t hits = 0;
-						auto post = [&](int i, int c, float fmv, float m)
-							{
-							const float score = __fsub_rn(ADD(fmv, m), total);
-							if (DUMP && i >= 1 && cpairs[kp] == P.dbg_pair)
-								{
-								P.dbg_bwd[(size_t)(i - 1)*LY + col0 + c] = m;
-								P.dbg_post[(size_t)(i - 1)*LY + col0 + c] =
-								  score < h.minScore ? 0.0f : (score >= 0.0f ? 1.0f : mb_expf_glibc(score));
-								}
-							return score;
-							};
-						// Backward cell from the row below ({M, IX, JX} of this column and M of the next one) and the
-						// IY / JY of the cell to the right
-						auto cell = [&](float mdiag, float vIX, float vJX, float riy, float rjy, float em, float eyc, float ex)
-							{
-							const float nM = ADD(mdiag, em);
-							const float nIX = ADD(vIX, ex);
-							const float nJX = ADD(vJX, ex);
-							const float nIY = ADD(riy, eyc);
-							const float nJY = ADD(rjy, eyc);
-							MbBwdCell r;
-							r.m = la(ADD(h.tMM, nM), la(ADD(h.tMI, nIX), la(ADD(h.tMJ, nJX),
-							  la(ADD(h.tMI, nIY), ADD(h.tMJ, nJY)))));
-							r.ix = la(ADD(h.tII, nIX), ADD(h.tIM, nM));
-							r.jx = la(ADD(h.tJJ, nJX), ADD(h.tJM, nM));
-							r.iy = la(ADD(h.tII, nIY), ADD(h.tIM, nM));
-							r.jy = la(ADD(h.tJJ, nJY), ADD(h.tJM, nM));
-							return r;
-							};
+						const bool dump = DUMP && cpairs[kp] == P.dbg_pair;
 						float4 *sp = st + lane;
 						const uint32_t *y2p = y2 + lane;
 						const float2 *fmc = fms + (size_t) t*W + lane;   // Forward M {row ia-1, row ia} of the lane's column 0
@@ -1152,9 +1125,9 @@ k_posterior_sm(const PostParams P)
 							const float2 f = *src;
 							const uint32_t yc = *y2p;
 							const float2 e = meb[yc];
-							const float sa = post(ia, c, f.y, h.tSM);
-							const MbBwdCell b = cell(mdiagb, h.tSI, h.tSJ, riyb, rjyb, e.x, e.y, exb);
-							const float sb = post(ia - 1, c, f.x, b.m);
+							const float sa = mb_post_score(P, dump, ia, LY, col0 + c, f.y, h.tSM, total);
+							const MbBwdCell b = mb_bwd_cell(h, la, mdiagb, h.tSI, h.tSJ, riyb, rjyb, e.x, e.y, exb);
+							const float sb = mb_post_score(P, dump, ia - 1, LY, col0 + c, f.x, b.m, total);
 							hits = (sa >= h.minScore ? 1u : 0u) + (sb >= h.minScore ? 0x10000u : 0u);
 							mdiaga = sp->x;
 							mdiagb = h.tSM;
@@ -1179,10 +1152,10 @@ k_posterior_sm(const PostParams P)
 							const uint32_t yc = *y2p;
 							const float2 e = mea[yc];                  // {match of row a, insert of Y}
 							const float emb = reinterpret_cast<const float *>(meb + yc)[0];
-							const MbBwdCell a = cell(mdiaga, v.y, v.z, riya, rjya, e.x, e.y, exa);
-							const float sa = post(ia, c, f.y, a.m);
-							const MbBwdCell b = cell(mdiagb, a.ix, a.jx, riyb, rjyb, emb, e.y, exb);
-							const float sb = post(ia - 1, c, f.x, b.m);
+							const MbBwdCell a = mb_bwd_cell(h, la, mdiaga, v.y, v.z, riya, rjya, e.x, e.y, exa);
+							const float sa = mb_post_score(P, dump, ia, LY, col0 + c, f.y, a.m, total);
+							const MbBwdCell b = mb_bwd_cell(h, la, mdiagb, a.ix, a.jx, riyb, rjyb, emb, e.y, exb);
+							const float sb = mb_post_score(P, dump, ia - 1, LY, col0 + c, f.x, b.m, total);
 							hits = 2u*hits + (sa >= h.minScore ? 1u : 0u) + (sb >= h.minScore ? 0x10000u : 0u);
 							mdiaga = v.x;
 							mdiagb = a.m;

@@ -1,21 +1,30 @@
-"""Per-cell instruction counts of the Forward / Backward column loops of every k_posterior_sm instantiation,
-for loops that compute R = 1 or 2 cells per iteration.
+"""Registers, stack bytes and the Forward / Backward column loops of every k_posterior_sm instantiation.
 
 Usage: python tests/sass_cells.py [library]   (default: muscle_b200/libmuscle_b200.so)
 
-The plain-mode passes compute two rows per lane per step, so their column loops hold 16 FFMA.RP (8 per
-LOG_ADD of each cell) and sass_loops.py, which looks for 8, finds none of them.  This script takes the
-innermost backward branches with 8*R FFMA.RP in their body; the first in the code is the Forward loop, the
-second the Backward loop.  For each it prints R, the loop's length in instructions, the FADD / FFMA.RP /
-LDS.128 / STS.128 / LDG counts per iteration, and the length per cell, the figure to compare across R.  Not
-a test: it reads the compiler's output.
+The plain-mode passes compute two rows per lane per step and the MEGA-mode passes one, so a column loop
+computes R = 2 or 1 cells per iteration.  A column loop is the innermost backward branch whose body holds
+8*R FFMA.RP (8 per LOG_ADD of each cell); the first in the code is the Forward loop, the second the Backward
+loop (any other number of such loops is reported with a warning and the loops are listed in code order).
+For each it prints R, the loop's length in instructions, the FADD / FFMA.RP / LDS.128 / STS.128 / LDG counts
+per iteration, and the length per cell, the figure to compare across R.  Not a test: it reads the
+compiler's output, and the counts are what a change to the kernel is checked against.
 """
 import os
 import re
 import subprocess
 import sys
 
-from sass_loops import COUNTED, INSN, KERNEL, ROOT, counted
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+INSN = re.compile(r"/\*([0-9a-f]{4,})\*/\s+(@!?U?P\w+\s+)?([A-Z][A-Z0-9_.]*)\s*([^;]*);")
+KERNEL = re.compile(r"_Z14k_posterior_smILb(\d)ELi(\d+)ELb(\d)EEv10PostParams")
+COUNTED = ("FADD", "FFMA.RP", "LDS.128", "STS.128", "LDG")
+
+
+def counted(op):
+	base = op.split(".")[0]
+	return {"FADD": base == "FADD", "FFMA.RP": op == "FFMA.RP", "LDS.128": base == "LDS" and op.endswith(".128"),
+	  "STS.128": base == "STS" and op.endswith(".128"), "LDG": base == "LDG"}
 
 
 def column_loops(insns):
