@@ -454,15 +454,12 @@ __global__ void k_densify(const DensifyJob *jobs, uint32_t njobs, uint32_t maxro
 // BuildPost
 struct BuildPostParams
 	{
-	uint32_t n;                                   // sequences in the store
 	uint32_t na, nb, cols_a, cols_b, ld;          // ld: row pitch of post
 	const uint32_t *ids_a, *ids_b;
 	const int32_t *col2pos_a;                     // [na][cols_a], -1 = gap
 	const uint32_t *p2c_b;                        // concatenated pos->col maps of B
 	const uint64_t *p2c_b_off;                    // [nb]
-	const uint64_t *rowbase;  const uint32_t *rowoff;  const mb200_entry *entries;
-	const uint64_t *trbase;   const uint32_t *troff;   const mb200_entry *trentries;
-	const uint64_t *entbase;
+	StoreView S;                                  // both orientations
 	float *post;                                  // cols_a x ld, zeroed
 	};
 
@@ -480,21 +477,6 @@ struct BpStage
 	                     // indexing by (column, s) would stage mostly gaps -- a 1000-row MSA of 350-residue
 	                     // proteins has 7000+ columns)
 	};
-
-__device__ __forceinline__ void bp_operand(const BuildPostParams &P, uint32_t a, uint32_t b, const uint32_t *&ro,
-  const mb200_entry *&en)
-	{
-	if (a < b)
-		{
-		const uint32_t q = mb_pair_index(P.n, a, b);
-		ro = P.rowoff + P.rowbase[q]; en = P.entries + P.entbase[q];
-		}
-	else
-		{
-		const uint32_t q = mb_pair_index(P.n, b, a);
-		ro = P.troff + P.trbase[q]; en = P.trentries + P.entbase[q];
-		}
-	}
 
 __global__ void __launch_bounds__(256)
 k_bp_gather(const BuildPostParams P, const BpStage G)
@@ -514,18 +496,16 @@ k_bp_gather(const BuildPostParams P, const BpStage G)
 			}
 		const uint32_t s = lo;
 		const uint32_t pos = r - G.rb[s];
-		const uint32_t *ro;
-		const mb200_entry *en;
-		bp_operand(P, P.ids_a[s], P.ids_b[t], ro, en);
-		const uint32_t e0 = ro[pos];
-		const uint32_t n = ro[pos + 1] - e0;
+		const StoreOperand o = mb_store_operand(P.S, P.ids_a[s], P.ids_b[t]);
+		const uint32_t e0 = o.ro[pos];
+		const uint32_t n = o.ro[pos + 1] - e0;
 		uint2 *dst = G.slots + idx*BP_W;
 		if (n <= BP_W)
 			{
 			const uint32_t *p2c = P.p2c_b + P.p2c_b_off[t];
 			for (uint32_t k = 0; k < n; ++k)
 				{
-				const mb200_entry v = en[e0 + k];
+				const mb200_entry v = o.en[e0 + k];
 				dst[k] = make_uint2(p2c[v.col], __float_as_uint(v.p));
 				}
 			for (uint32_t k = n; k < BP_W; ++k)
@@ -684,14 +664,12 @@ k_bp_apply(const BuildPostParams P, const BpStage G, const BpSched S)
 						else if (lane == 0)
 							{
 							// rare: more than BP_W entries in the sparse row -> gather directly, still in order
-							const uint32_t *ro;
-							const mb200_entry *en;
-							bp_operand(P, P.ids_a[s], P.ids_b[t0 + l], ro, en);
+							const StoreOperand o = mb_store_operand(P.S, P.ids_a[s], P.ids_b[t0 + l]);
 							const uint32_t *p2c = P.p2c_b + P.p2c_b_off[t0 + l];
-							for (uint32_t e = ro[pos]; e < ro[pos + 1]; ++e)
+							for (uint32_t e = o.ro[pos]; e < o.ro[pos + 1]; ++e)
 								{
-								const uint32_t a = accA + p2c[en[e].col]*4;
-								sts_f32(a, __fadd_rn(lds_f32(a), en[e].p));
+								const uint32_t a = accA + p2c[o.en[e].col]*4;
+								sts_f32(a, __fadd_rn(lds_f32(a), o.en[e].p));
 								}
 							}
 						__syncwarp();
@@ -908,7 +886,8 @@ struct BpCells
 	const uint32_t *rowof;       // [residues of A] column of A's alignment = row of post
 	const uint32_t *seqof;       // [residues of A] member of A that owns the residue
 	uint32_t *cnt;               // [(residue of the batch) x nb] terms of the pair's sparse row
-	uint64_t *eptr;              // [same] first entry of that sparse row: index into entries, bit 63 = transposed store
+	uint64_t *eptr;              // [same] first entry of that sparse row: index into the entries of its side of the
+	                             // store, bit 63 = the transposed side
 	const uint32_t *off;         // exclusive scan of cnt (one more entry than cnt)
 	const uint32_t *base;        // [residue of the batch] first term of the residue in (row, s) order
 	uint32_t colbits;            // key = row << colbits | col
@@ -941,25 +920,11 @@ __global__ void k_bpc_count(const BuildPostParams P, const BpCells G)
 		const uint32_t r = r0 + (uint32_t)(idx/P.nb);
 		const uint32_t s = G.seqof[r];
 		const uint32_t pos = r - G.rb[s];
-		const uint32_t a = P.ids_a[s], b = P.ids_b[t];
-		uint32_t e0, e1;
-		uint64_t ep;
-		if (a < b)
-			{
-			const uint32_t q = mb_pair_index(P.n, a, b);
-			const uint32_t *ro = P.rowoff + P.rowbase[q];
-			e0 = ro[pos]; e1 = ro[pos + 1];
-			ep = P.entbase[q] + e0;
-			}
-		else
-			{
-			const uint32_t q = mb_pair_index(P.n, b, a);
-			const uint32_t *ro = P.troff + P.trbase[q];
-			e0 = ro[pos]; e1 = ro[pos + 1];
-			ep = (P.entbase[q] + e0) | (1ull << 63);
-			}
+		const StoreOperand o = mb_store_operand(P.S, P.ids_a[s], P.ids_b[t]);
+		const uint32_t e0 = o.ro[pos], e1 = o.ro[pos + 1];
+		const mb200_entry *side = o.transposed ? P.S.tr.entries : P.S.fwd.entries;
 		G.cnt[idx] = e1 - e0;
-		G.eptr[idx] = ep;
+		G.eptr[idx] = (uint64_t)(o.en + e0 - side) | ((uint64_t) o.transposed << 63);
 		}
 	}
 
@@ -978,7 +943,7 @@ __global__ void k_bpc_emit(const BuildPostParams P, const BpCells G)
 		const uint32_t t = (uint32_t)(idx % P.nb);
 		const uint32_t rl = (uint32_t)(idx/P.nb);
 		const uint64_t ep = G.eptr[idx];
-		const mb200_entry *en = ((ep >> 63) ? P.trentries : P.entries) + (ep & ~(1ull << 63));
+		const mb200_entry *en = ((ep >> 63) ? P.S.tr.entries : P.S.fwd.entries) + (ep & ~(1ull << 63));
 		const uint32_t *p2c = P.p2c_b + P.p2c_b_off[t];
 		const uint32_t kbase = G.rowof[r0 + rl] << G.colbits;
 		const uint32_t o = G.base[rl] + (G.off[idx] - G.off[(uint64_t) rl*P.nb]);
@@ -1182,12 +1147,13 @@ struct JoinMembers
 	uint32_t *d_ids = nullptr, *d_rb = nullptr, *d_p2cb = nullptr;
 	uint64_t *d_boff = nullptr;
 	int32_t *d_c2p = nullptr;
+	StoreView store;                 // both orientations of the all-pairs store
 	};
 // Checks the store and that every id is in range and listed once (A and B disjoint); builds the host maps
 static int join_members(mb200_ctx *ctx, const char *who, uint32_t na, const uint32_t *ids_a, uint32_t nb, const uint32_t *ids_b,
   JoinMembers &M)
 	{
-	const int rc = mb_store_require(ctx, who, NEED_ALLPAIRS | FORM_TRANSPOSED);
+	const int rc = mb_store_view(ctx, who, NEED_ALLPAIRS | FORM_TRANSPOSED, &M.store);
 	if (rc != MB200_OK)
 		return rc;
 	M.na = na; M.nb = nb;
@@ -1469,13 +1435,9 @@ static int join_core(mb200_ctx *ctx, const JoinMembers &M, uint32_t cols_a, uint
 	CU(cudaMemsetAsync(scratch, 0, L.dense_bytes, st));
 
 	BuildPostParams P;
-	P.n = ctx->nseq; P.na = na; P.nb = nb; P.cols_a = cols_a; P.cols_b = cols_b; P.ld = L.ld;
+	P.na = na; P.nb = nb; P.cols_a = cols_a; P.cols_b = cols_b; P.ld = L.ld;
 	P.ids_a = M.d_ids; P.ids_b = M.d_ids + na; P.col2pos_a = M.d_c2p; P.p2c_b = M.d_p2cb; P.p2c_b_off = M.d_boff;
-	P.rowbase = (const uint64_t *) ctx->d_rowbase.p; P.rowoff = (const uint32_t *) ctx->d_rowoff.p;
-	P.entries = (const mb200_entry *) ctx->d_entries.p;
-	P.trbase = (const uint64_t *) ctx->d_tr_rowbase.p; P.troff = (const uint32_t *) ctx->d_tr_rowoff.p;
-	P.trentries = (const mb200_entry *) ctx->d_tr_entries.p;
-	P.entbase = (const uint64_t *) ctx->d_entbase.p;
+	P.S = M.store;
 	P.post = (float *) pr.dense;
 	// large joins: bucket the contributions by cell (see k_bpc_*); small ones: ordered row walk (k_bp_apply)
 	const char *ev_sort = getenv("MB200_BP_SORT_MIN");             // tuning hook: (residues of A) x |B| from which to sort

@@ -40,6 +40,55 @@ __host__ __device__ __forceinline__ uint32_t mb_pair_index(uint32_t n, uint32_t 
 	return (uint32_t)((uint64_t) a*n - (uint64_t) a*(a + 1)/2 + (b - a - 1));
 	}
 
+// Device view of an all-pairs store (mb_store_view).  Pair (a,b), a < b, is kept once, at mb_pair_index(n, a, b),
+// in two orientations that share entbase: the forward one (rows = positions of a) and the transposed one
+// (rows = positions of b).  Row i of pair q in one orientation has the entries rowoff[rowbase[q] + i] ..
+// rowoff[rowbase[q] + i + 1] - 1 of entries + entbase[q] and, once the column masks are built, the header
+// hdr[rowbase[q] + i] into words.
+struct StoreSide
+	{
+	const uint64_t *rowbase;
+	const uint32_t *rowoff;
+	const mb200_entry *entries;
+	const uint2 *hdr, *words;          // null unless the view was asked for FORM_MASKED
+	};
+struct StoreView
+	{
+	uint32_t n;                        // sequences
+	const uint64_t *entbase;
+	StoreSide fwd, tr;                 // tr is null unless the view was asked for FORM_TRANSPOSED or more
+	};
+// one pair's posteriors with rows = positions of sequence a and columns = positions of sequence b
+struct StoreOperand
+	{
+	const uint32_t *ro;                // row offsets into en
+	const mb200_entry *en;
+	const uint2 *hdr, *words;          // column masks of the rows (not to be read from a view without masks)
+	bool transposed;                   // read from the transposed orientation
+	};
+// a < b: the forward orientation of pair (a,b); a > b: the transposed orientation of pair (b,a).  Each branch
+// assigns the fields itself: through a helper that returns the record, nvcc no longer sees that the pointers
+// are global and the kernels read through them with generic loads.
+__device__ __forceinline__ StoreOperand mb_store_operand(const StoreView &V, uint32_t a, uint32_t b)
+	{
+	StoreOperand o;
+	if (a < b)
+		{
+		const uint32_t q = mb_pair_index(V.n, a, b);
+		const uint64_t rb = V.fwd.rowbase[q];
+		o.ro = V.fwd.rowoff + rb; o.en = V.fwd.entries + V.entbase[q]; o.hdr = V.fwd.hdr + rb; o.words = V.fwd.words;
+		o.transposed = false;
+		}
+	else
+		{
+		const uint32_t q = mb_pair_index(V.n, b, a);
+		const uint64_t rb = V.tr.rowbase[q];
+		o.ro = V.tr.rowoff + rb; o.en = V.tr.entries + V.entbase[q]; o.hdr = V.tr.hdr + rb; o.words = V.tr.words;
+		o.transposed = true;
+		}
+	return o;
+	}
+
 struct MbHmm
 	{
 	float tSM, tSI, tSJ, tMM, tMI, tMJ, tII, tIM, tJJ, tJM;   // hmmscores.h:1-13

@@ -133,6 +133,7 @@ void mb_store_drop(mb200_ctx *ctx);
 void mb_store_fresh(mb200_ctx *ctx, bool adopted);
 void mb_store_values_written(mb200_ctx *ctx);
 int mb_store_require(mb200_ctx *ctx, const char *who, unsigned needs);
+int mb_store_view(mb200_ctx *ctx, const char *who, unsigned needs, StoreView *v);
 void mb_store_entry_range(const mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi, uint64_t *e_lo, uint64_t *e_hi);
 int mb_build_masks(mb200_ctx *ctx);             // relax.cu
 void mb_release_post_scratch(mb200_ctx *ctx);

@@ -32,7 +32,6 @@
 #include <cub/cub.cuh>
 #include <thrust/iterator/transform_iterator.h>
 #include <algorithm>
-#include <cstdlib>
 #include <cstring>
 
 // ---------------------------------------------------------------------------------------------
@@ -169,15 +168,11 @@ int mb_build_masks(mb200_ctx *ctx)
 // ---------------------------------------------------------------------------------------------
 struct RelaxParams
 	{
-	uint32_t n;                       // sequences
 	uint32_t nwork;                   // pairs to update
 	const uint32_t *order;            // work list: all-pairs indexes in 2-D tile order
 	const uint32_t *seqlen;
-	const uint64_t *rowbase;  const uint32_t *rowoff;  const mb200_entry *entries;      // forward
-	const uint64_t *trbase;   const mb200_entry *trentries;                             // transposed
-	const uint2 *hdr, *words, *trhdr, *trwords;                                         // column masks
-	const uint64_t *entbase;
-	mb200_entry *out;                 // new values (same layout as entries)
+	StoreView S;                      // both orientations with their column masks
+	mb200_entry *out;                 // new values (same layout as S.fwd.entries)
 	};
 
 // operands of one z: S[x->z] (rows = positions of x) and S[y->z] (rows = positions of y)
@@ -193,11 +188,9 @@ struct ZDesc
 #define RELAX_EPT 4          // entries per thread held in registers per sweep
 #endif
 
-// MINB: resident CTAs/SM the register allocation is bounded for (sm_90a: 2: 96 registers, no spill;
-// 3: 80, no spill; 4: 64, 56 bytes spilled).  The kernel is bound by gather latency, so occupancy
-// wins over spills; 4 is the default (MB200_RELAX_OCC selects another).
-template <int MINB>
-__global__ void __launch_bounds__(RELAX_THREADS, MINB)
+// Bounded for 4 resident CTAs/SM: 64 registers on sm_90a with 56 bytes spilled (2 CTAs: 96 registers and
+// 3 CTAs: 80, neither spills).  The kernel is bound by gather latency, so occupancy wins over spills.
+__global__ void __launch_bounds__(RELAX_THREADS, 4)
 k_relax(const RelaxParams P)
 	{
 	__shared__ ZDesc zd[RELAX_ZCHUNK];
@@ -205,7 +198,7 @@ k_relax(const RelaxParams P)
 		return;
 	const uint32_t p = P.order[blockIdx.x];
 	// invert p -> (x,y): find x with base(x) <= p < base(x+1)
-	const uint32_t n = P.n;
+	const uint32_t n = P.S.n;
 	uint32_t x = 0;
 		{
 		// base(x) = x*n - x(x+1)/2 ; solve by a short search from the analytic estimate
@@ -219,9 +212,9 @@ k_relax(const RelaxParams P)
 		}
 	const uint32_t y = x + 1 + (p - (uint32_t)((uint64_t) x*n - (uint64_t) x*(x + 1)/2));
 	const uint32_t LX = P.seqlen[x];
-	const uint32_t *ro = P.rowoff + P.rowbase[p];
-	const uint64_t eb = P.entbase[p];
-	const mb200_entry *en = P.entries + eb;
+	const uint32_t *ro = P.S.fwd.rowoff + P.S.fwd.rowbase[p];
+	const uint64_t eb = P.S.entbase[p];
+	const mb200_entry *en = P.S.fwd.entries + eb;
 	mb200_entry *out = P.out + eb;
 	const uint32_t nnz = ro[LX];
 	const float fn = (float) n;
@@ -263,28 +256,9 @@ k_relax(const RelaxParams P)
 				d.hdrA = nullptr;
 				if (z < n && z != x && z != y)
 					{
-					// S[x->z]: rows are positions of x
-					if (x < z)
-						{
-						const uint32_t q = mb_pair_index(n, x, z);
-						d.hdrA = P.hdr + P.rowbase[q]; d.wordsA = P.words; d.enA = P.entries + P.entbase[q];
-						}
-					else
-						{
-						const uint32_t q = mb_pair_index(n, z, x);
-						d.hdrA = P.trhdr + P.trbase[q]; d.wordsA = P.trwords; d.enA = P.trentries + P.entbase[q];
-						}
-					// S[y->z]: rows are positions of y
-					if (y < z)
-						{
-						const uint32_t q = mb_pair_index(n, y, z);
-						d.hdrB = P.hdr + P.rowbase[q]; d.wordsB = P.words; d.enB = P.entries + P.entbase[q];
-						}
-					else
-						{
-						const uint32_t q = mb_pair_index(n, z, y);
-						d.hdrB = P.trhdr + P.trbase[q]; d.wordsB = P.trwords; d.enB = P.trentries + P.entbase[q];
-						}
+					const StoreOperand A = mb_store_operand(P.S, x, z), B = mb_store_operand(P.S, y, z);
+					d.hdrA = A.hdr; d.wordsA = A.words; d.enA = A.en;
+					d.hdrB = B.hdr; d.wordsB = B.words; d.enB = B.en;
 					}
 				zd[threadIdx.x] = d;
 				}
@@ -405,17 +379,11 @@ __global__ void k_copy_entries(uint64_t lo, uint64_t hi, const mb200_entry *__re
 static int prepare_relax_order(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi)
 	{
 	const uint32_t n = ctx->nseq;
-	static uint32_t tile = 0;
-	if (tile == 0)
-		{
-		const char *ev = getenv("MB200_RELAX_TILE");           // tuning hook
-		tile = ev ? (uint32_t) std::max(1, atoi(ev)) : RELAX_TILE;
-		}
 	if (ctx->relax_order_n == n && ctx->relax_order_lo == p_lo && ctx->relax_order_hi == p_hi && ctx->d_relax_order.p)
 		return MB200_OK;
 	std::vector<uint32_t> order;
 	order.reserve(p_hi - p_lo);
-	const uint32_t T = tile;
+	const uint32_t T = RELAX_TILE;
 	for (uint32_t tx = 0; tx < n; tx += T)
 		for (uint32_t ty = tx; ty < n; ty += T)
 			for (uint32_t x = tx; x < std::min(n, tx + T); ++x)
@@ -453,7 +421,9 @@ int mb200_consistency_iter(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi)
 	cudaSetDevice(ctx->device);
 	cudaStream_t st = ctx->stream;
 	CU(cudaEventRecord(ctx->ev0, st));
-	rc = mb_store_require(ctx, "mb200_consistency_iter", NEED_ALLPAIRS | FORM_MASKED);
+	// after ev0: building the transposed orientation and the masks counts in last_total_ms
+	RelaxParams P;
+	rc = mb_store_view(ctx, "mb200_consistency_iter", NEED_ALLPAIRS | FORM_MASKED, &P.S);
 	if (rc != MB200_OK)
 		return rc;
 	ENSURE(ctx->d_entries2, (ctx->store_nnz + 64)*sizeof(mb200_entry));
@@ -463,32 +433,12 @@ int mb200_consistency_iter(mb200_ctx *ctx, uint32_t p_lo, uint32_t p_hi)
 		rc = prepare_relax_order(ctx, p_lo, p_hi);
 		if (rc != MB200_OK)
 			return rc;
-		RelaxParams P;
-		P.n = n; P.nwork = p_hi - p_lo;
+		P.nwork = p_hi - p_lo;
 		P.order = (const uint32_t *) ctx->d_relax_order.p;
 		P.seqlen = (const uint32_t *) ctx->d_seqlen.p;
-		P.rowbase = (const uint64_t *) ctx->d_rowbase.p;
-		P.rowoff = (const uint32_t *) ctx->d_rowoff.p;
-		P.entries = (const mb200_entry *) ctx->d_entries.p;
-		P.trbase = (const uint64_t *) ctx->d_tr_rowbase.p;
-		P.trentries = (const mb200_entry *) ctx->d_tr_entries.p;
-		P.hdr = (const uint2 *) ctx->d_mk_hdr.p; P.words = (const uint2 *) ctx->d_mk_words.p;
-		P.trhdr = (const uint2 *) ctx->d_tr_mk_hdr.p; P.trwords = (const uint2 *) ctx->d_tr_mk_words.p;
-		P.entbase = (const uint64_t *) ctx->d_entbase.p;
 		P.out = (mb200_entry *) ctx->d_entries2.p;
 		CU(cudaEventRecord(ctx->ev1, st));
-		static int occ = 0;
-		if (occ == 0)
-			{
-			const char *ev = getenv("MB200_RELAX_OCC");        // tuning hooks
-			occ = ev ? atoi(ev) : 4;
-			}
-		if (occ == 2)
-			k_relax<2><<<p_hi - p_lo, RELAX_THREADS, 0, st>>>(P);
-		else if (occ == 4)
-			k_relax<4><<<p_hi - p_lo, RELAX_THREADS, 0, st>>>(P);
-		else
-			k_relax<3><<<p_hi - p_lo, RELAX_THREADS, 0, st>>>(P);
+		k_relax<<<p_hi - p_lo, RELAX_THREADS, 0, st>>>(P);
 		CU(cudaGetLastError());
 		ctx->stats.kernel_launches++;
 		}

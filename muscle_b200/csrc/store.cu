@@ -1,6 +1,7 @@
 // store.cu -- the device-resident sparse posterior store: its state (StoreState, engine.h), packing in
 // pair order (export and the multi-GPU exchange image), loading a gathered image, values-only views,
-// and the transposed orientation that the consistency kernel and the joins need.
+// and the transposed orientation that the consistency kernel and the joins need, with the view of both
+// orientations those kernels read (StoreView, common.cuh).
 //
 // Reference counterparts: the store replaces MPCFlat::m_SparsePosts1/2 (mpcflat.h:46-49); the wire
 // format of one pair is MySparseMx's (mysparsemx.h:6-98).  The transposed orientation replaces the
@@ -380,6 +381,36 @@ int mb_store_require(mb200_ctx *ctx, const char *who, unsigned needs)
 		}
 	if ((needs & NEED_INDEX) && !s.index_valid && (rc = read_index(ctx, true)) != MB200_OK)
 		return rc;
+	return MB200_OK;
+	}
+
+// mb_store_require(needs), then the kernels' view of the store: the transposed side is filled when `needs`
+// asks for FORM_TRANSPOSED or more, the column masks when it asks for FORM_MASKED
+int mb_store_view(mb200_ctx *ctx, const char *who, unsigned needs, StoreView *v)
+	{
+	const int rc = mb_store_require(ctx, who, needs);
+	if (rc != MB200_OK)
+		return rc;
+	const unsigned want = needs & 3;
+	*v = StoreView{};
+	v->n = ctx->nseq;
+	v->entbase = (const uint64_t *) ctx->d_entbase.p;
+	v->fwd.rowbase = (const uint64_t *) ctx->d_rowbase.p;
+	v->fwd.rowoff = (const uint32_t *) ctx->d_rowoff.p;
+	v->fwd.entries = (const mb200_entry *) ctx->d_entries.p;
+	if (want >= FORM_TRANSPOSED)
+		{
+		v->tr.rowbase = (const uint64_t *) ctx->d_tr_rowbase.p;
+		v->tr.rowoff = (const uint32_t *) ctx->d_tr_rowoff.p;
+		v->tr.entries = (const mb200_entry *) ctx->d_tr_entries.p;
+		}
+	if (want == FORM_MASKED)
+		{
+		v->fwd.hdr = (const uint2 *) ctx->d_mk_hdr.p;
+		v->fwd.words = (const uint2 *) ctx->d_mk_words.p;
+		v->tr.hdr = (const uint2 *) ctx->d_tr_mk_hdr.p;
+		v->tr.words = (const uint2 *) ctx->d_tr_mk_words.p;
+		}
 	return MB200_OK;
 	}
 

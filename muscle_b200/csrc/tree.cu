@@ -93,7 +93,7 @@ k_upgma(const UpgmaParams P)
 			if (m == i)
 				continue;
 			const uint32_t a = min(i, m), b = max(i, m);
-			const float e = P.ea[(uint64_t) a*n - (uint64_t) a*(a + 1)/2 + (b - a - 1)];
+			const float e = P.ea[mb_pair_index(n, a, b)];
 			if (!(e >= 0.0f && e <= 1.0f))
 				*P.err = 1;                                  // the reference asserts 0 <= EA <= 1 (upgma5.cpp:512)
 			const float d = __fsub_rn(1.0f, e);
