@@ -238,6 +238,18 @@ int mb200_debug_plan(mb200_ctx *ctx, uint32_t *npairs, uint32_t *nchains, uint32
 int mb200_calc_post_dense_pair(mb200_ctx *ctx, uint32_t npairs, const uint32_t *pair_x, const uint32_t *pair_y,
                                uint32_t which, float *post_out, float *fwd_m_out, float *bwd_m_out,
                                float *total_out);
+/* Evaluate one of k_posterior_sm's per-score primitives on n inputs, with the kernel's own device code:
+ *   MB200_MATH_LOG_ADD     out[k] = LOG_ADD(a[k], b[k])   (scoretype.h:120-124)
+ *   MB200_MATH_LOG_ADD_BA  out[k] = LOG_ADD(b[k], a[k])
+ *   MB200_MATH_POST_PROB   out[k] = the probability of posterior score a[k], 0 below min_sparse_score
+ *                          (calcposteriorflat.cpp:15-20)
+ *   MB200_MATH_KEEP        out[k] = 1.0f if a cell of score a[k] is kept in the sparse store, else 0.0f
+ * a == NULL: a[k] = the float whose bits are a_first_bits + k (formed on the device); b == NULL: b[k] =
+ * b_scalar.  The POST_PROB and KEEP ops read min_sparse_score of mb200_set_hmm.  Host arrays; the work runs
+ * in chunks through one buffer the context keeps.  Never touches the store. */
+enum { MB200_MATH_LOG_ADD = 0, MB200_MATH_LOG_ADD_BA = 1, MB200_MATH_POST_PROB = 2, MB200_MATH_KEEP = 3 };
+int mb200_debug_math(mb200_ctx *ctx, int op, uint64_t n, const float *a, uint32_t a_first_bits,
+                     const float *b, float b_scalar, float *out);
 
 /* ---- several GPUs from one process (SURVEY.md section 8b: "mb200_create(ndev, ...)") -------- */
 /* A group is ndev single-device contexts plus the two exchange steps of the path (section 8e).

@@ -215,6 +215,21 @@ __device__ __forceinline__ float mb_expf_glibc(float x)
 	return __double2float_rn(y);
 	}
 
+// probability of a candidate posterior score, score >= minScore (calcposteriorflat.cpp:19-20)
+__device__ __forceinline__ float mb_post_prob(float score)
+	{
+	return score >= 0.0f ? 1.0f : mb_expf_glibc(score);
+	}
+
+// least posterior score whose cell is kept in the sparse store.  A cell is kept when its probability is
+// >= 0.01f (mysparsemx.cpp:139-141), and for every float s in [-10, 0] glibc's expf(s) >= 0.01f exactly
+// when s >= -4.60517025f (0xc0935d8e, itself logf(0.01f)), so the kept decision is a compare of the score
+// with this; a larger minScore cuts first.
+__device__ __forceinline__ float mb_keep_score(const MbHmm &h)
+	{
+	return fmaxf(h.minScore, __uint_as_float(0xc0935d8eu));
+	}
+
 // head of k_posterior_sm's dynamic shared memory; the emission tables and the warps' state follow it
 struct PostSmemHdr
 	{

@@ -127,7 +127,7 @@ void mb200_destroy(mb200_ctx *ctx)
 	  &ctx->d_ea, &ctx->d_dbg, &ctx->d_pack_off, &ctx->d_pack_ent, &ctx->d_entries2,
 	  &ctx->d_tr_rowoff, &ctx->d_tr_rowbase, &ctx->d_tr_entries, &ctx->d_tr_perm,
 	  &ctx->d_tmp, &ctx->d_tmp2, &ctx->d_mk_hdr, &ctx->d_mk_words, &ctx->d_tr_mk_hdr, &ctx->d_tr_mk_words,
-	  &ctx->d_relax_order, &ctx->d_p2c, &ctx->d_join, &ctx->d_stage, &ctx->d_megaT, &ctx->d_insP };
+	  &ctx->d_relax_order, &ctx->d_p2c, &ctx->d_join, &ctx->d_stage, &ctx->d_megaT, &ctx->d_insP, &ctx->d_math };
 	if (ctx->h_pinned)
 		cudaFreeHost(ctx->h_pinned);
 	for (DevBuf *b : bufs)

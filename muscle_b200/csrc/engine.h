@@ -115,6 +115,7 @@ struct mb200_ctx
 	cudaStream_t aux[kStreams] = {};
 	cudaEvent_t aux_done[kStreams] = {};
 	DevBuf d_dbg;
+	DevBuf d_math;                    // mb200_debug_math: one chunk of operands and results (math.cu)
 	int debug_force_c = 0;
 	int occ_cache[MB_MAX_C + 1] = {}, occ_cache_k = -1;     // resident CTAs/SM of k_posterior_sm per size class
 	};

@@ -174,8 +174,7 @@ __device__ __forceinline__ float mb_post_score(const PostParams &P, bool dump, i
 	if (dump && i >= 1)
 		{
 		P.dbg_bwd[(size_t)(i - 1)*LY + col] = m;
-		P.dbg_post[(size_t)(i - 1)*LY + col] =
-		  score < P.h.minScore ? 0.0f : (score >= 0.0f ? 1.0f : mb_expf_glibc(score));
+		P.dbg_post[(size_t)(i - 1)*LY + col] = score < P.h.minScore ? 0.0f : mb_post_prob(score);
 		}
 	return score;
 	}
@@ -323,7 +322,7 @@ __device__ void mb_compact_ea(const PostParams &P, uint32_t pair, int LX, int LY
 					if (idx >= 0)
 						{
 						ent = row[idx];             // {score, column}: the probability (calcposteriorflat.cpp:20)
-						ent.p = ent.p >= 0.0f ? 1.0f : mb_expf_glibc(ent.p);
+						ent.p = mb_post_prob(ent.p);
 						}
 					const bool keep = idx >= 0 && ent.p >= 0.01f;          // mysparsemx.cpp:139-141
 					const uint32_t b = __ballot_sync(MB_FULL, keep);
@@ -368,7 +367,7 @@ __device__ void mb_compact_ea(const PostParams &P, uint32_t pair, int LX, int LY
 			if (has)
 				{
 				ent = prow[(size_t)(i - 1 + r)*MB_CAP + rcnt - 1 - (lane - rex)];
-				ent.p = ent.p >= 0.0f ? 1.0f : mb_expf_glibc(ent.p);
+				ent.p = mb_post_prob(ent.p);
 				}
 			const bool keep = has && ent.p >= 0.01f;
 			const uint32_t b = __ballot_sync(MB_FULL, keep);
@@ -430,7 +429,7 @@ __device__ void mb_compact_ea(const PostParams &P, uint32_t pair, int LX, int LY
 					if (idx >= 0)
 						{
 						ent = row[idx];             // {score, column}: the probability (calcposteriorflat.cpp:20)
-						ent.p = ent.p >= 0.0f ? 1.0f : mb_expf_glibc(ent.p);
+						ent.p = mb_post_prob(ent.p);
 						}
 					const int lc = (int) ent.col - j0;
 					if (idx >= 0 && lc >= 0 && lc < W)
@@ -878,12 +877,13 @@ k_posterior_sm(const PostParams P)
 		// which any lane has one (under SIMT a branch costs the whole warp when one lane takes it).  The
 		// list holds scores, not probabilities: expf is a long FP64 chain, and the compaction forms p
 		// from 32 converged lanes instead.  A candidate is kept when p >= 0.01f (mysparsemx.cpp:139-141),
-		// and for every float s in [-10, 0] glibc's expf(s) >= 0.01f exactly when s >= -4.60517025f
-		// (0xc0935d8e, itself logf(0.01f); checked on all 1.09e9 of them), so the kept count is a compare
-		// of the score.  Row i's entry count travels with the wavefront like the state: lane l+1 finished
-		// its columns of row i, which lie to the right, one step before lane l, so the list stays in
-		// descending column order; across strips the count rides in the spare .w of the edge record, and
-		// lane 0 of strip 0, the last to touch the row, stores it in rowcnt.
+		// which is a compare of the score with mb_keep_score (tests/test_logadd_expf_gpu.py checks the two
+		// decisions agree on every score).  Row i's entry count travels with the wavefront like the state:
+		// lane l+1 finished its columns of row i, which lie to the right, one step before lane l, so the
+		// list stays in descending column order; across strips the count rides in the spare .w of the edge
+		// record, and lane 0 of strip 0, the last to touch the row, stores it in rowcnt.  The threshold is
+		// mb_keep_score's expression written out: called through the helper, ptxas assigns two registers
+		// of the plain kernels differently.
 		const float keepScore = fmaxf(h.minScore, __uint_as_float(0xc0935d8eu));
 		uint32_t kept = 0;
 		bool overflow = false;

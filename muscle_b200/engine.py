@@ -23,8 +23,11 @@ EXPORTS = [
 	"mb200_group_create", "mb200_group_destroy", "mb200_group_last_error", "mb200_group_size", "mb200_group_ctx",
 	"mb200_group_set_hmm", "mb200_group_set_seqs", "mb200_group_posteriors_allpairs", "mb200_group_consistency_iter",
 	"mb200_group_get_stats", "mb200_msa_reset", "mb200_msa_join", "mb200_msa_export", "mb200_guide_tree", "mb200_set_seqs_mega",
-	"mb200_group_set_seqs_mega",
+	"mb200_group_set_seqs_mega", "mb200_debug_math",
 ]
+
+# ops of mb200_debug_math
+MATH_LOG_ADD, MATH_LOG_ADD_BA, MATH_POST_PROB, MATH_KEEP = 0, 1, 2, 3
 
 
 class MB200Error(RuntimeError):
@@ -68,6 +71,8 @@ def load_library():
 		L.mb200_group_destroy.argtypes = [C.c_void_p]
 		L.mb200_group_destroy.restype = None
 		L.mb200_group_size.argtypes = [C.c_void_p]
+		L.mb200_debug_math.argtypes = [C.c_void_p, C.c_int, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p, C.c_float,
+		  C.c_void_p]
 		_lib = L
 	return _lib
 
@@ -242,6 +247,19 @@ class Engine(_Inputs):
 		  _ptr(bin_start), _ptr(limits)))
 		return {"order": order, "chain": chain, "bin_start": bin_start, "chain_rows": int(limits[0]),
 		  "chain_pairs": int(limits[1])}
+
+	def debug_math(self, op, n=None, a=None, a_first_bits=0, b=None, b_scalar=0.0):
+		"""one of k_posterior_sm's per-score primitives (MATH_*) on n inputs -> float32[n]; a None: the floats
+		whose bits are a_first_bits .. a_first_bits + n - 1; b None: b_scalar"""
+		a = None if a is None else np.ascontiguousarray(a, np.float32)
+		b = None if b is None else np.ascontiguousarray(b, np.float32)
+		if n is None:
+			n = len(a)
+		assert (a is None or len(a) == n) and (b is None or len(b) == n)
+		out = np.empty(n, np.float32)
+		self._ck(self.lib.mb200_debug_math(self.h, int(op), n, _ptr(a), a_first_bits & 0xffffffff, _ptr(b),
+		  float(np.float32(b_scalar)), _ptr(out)))
+		return out
 
 	def set_nnz_per_row_cap(self, cap):
 		self._ck(self.lib.mb200_set_nnz_per_row_cap(self.h, C.c_uint32(cap)))

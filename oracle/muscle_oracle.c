@@ -222,6 +222,14 @@ float mo_total(const float *fwd, const float *bwd, uint32_t LX, uint32_t LY)
 	return sum;
 	}
 
+/* calcposteriorflat.cpp:15-20: the probability CalcPostFlat writes for one posterior score */
+static float post_prob(float score, float min_score)
+	{
+	if (score < min_score)
+		return 0.0f;
+	return (score >= 0.0f) ? 1.0f : expf(score);
+	}
+
 /* calcposteriorflat.cpp:4-27 */
 void mo_post(const mo_hmm *h, const float *fwd, const float *bwd, uint32_t LX, uint32_t LY, float *post)
 	{
@@ -230,11 +238,47 @@ void mo_post(const mo_hmm *h, const float *fwd, const float *bwd, uint32_t LX, u
 		for (uint32_t j = 1; j <= LY; ++j)
 			{
 			const float score = CELL(fwd, i, j, LY + 1)[MO_M] + CELL(bwd, i, j, LY + 1)[MO_M] - total;
-			float p = 0.0f;
-			if (!(score < h->min_sparse_score))
-				p = (score >= 0.0f) ? 1.0f : expf(score);
-			post[(size_t)(i - 1)*LY + (j - 1)] = p;
+			post[(size_t)(i - 1)*LY + (j - 1)] = post_prob(score, h->min_sparse_score);
 			}
+	}
+
+/* batch and bit-range forms of mo_log_add and post_prob for the arithmetic sweeps of the tests */
+static float bits_float(uint32_t u)
+	{
+	float f;
+	memcpy(&f, &u, 4);
+	return f;
+	}
+
+void mo_log_add_n(uint64_t n, const float *a, const float *b, float *out)
+	{
+#pragma omp parallel for schedule(static)
+	for (int64_t k = 0; k < (int64_t) n; ++k)
+		out[k] = mo_log_add(a[k], b[k]);
+	}
+
+void mo_log_add_range(uint64_t n, uint32_t a_first_bits, float b, int swap, float *out)
+	{
+#pragma omp parallel for schedule(static)
+	for (int64_t k = 0; k < (int64_t) n; ++k)
+		{
+		const float a = bits_float(a_first_bits + (uint32_t) k);
+		out[k] = swap ? mo_log_add(b, a) : mo_log_add(a, b);
+		}
+	}
+
+void mo_post_prob_n(uint64_t n, const float *s, float min_score, float *out)
+	{
+#pragma omp parallel for schedule(static)
+	for (int64_t k = 0; k < (int64_t) n; ++k)
+		out[k] = post_prob(s[k], min_score);
+	}
+
+void mo_post_prob_range(uint64_t n, uint32_t s_first_bits, float min_score, float *out)
+	{
+#pragma omp parallel for schedule(static)
+	for (int64_t k = 0; k < (int64_t) n; ++k)
+		out[k] = post_prob(bits_float(s_first_bits + (uint32_t) k), min_score);
 	}
 
 /* calcpost.cpp:4-36 minus the label registry */

@@ -34,6 +34,13 @@ typedef struct { float p; uint32_t col; } mo_entry;   /* MySparseMx wire format,
 
 float mo_logexp1(float x);
 float mo_log_add(float x, float y);
+/* batch forms (OpenMP): out[k] = mo_log_add(a[k], b[k]); out[k] = the probability CalcPostFlat writes for
+ * score s[k] (calcposteriorflat.cpp:15-20, libm expf).  Range forms: a[k] / s[k] is the float whose bits are
+ * first_bits + k; swap: out[k] = mo_log_add(b, a[k]). */
+void  mo_log_add_n(uint64_t n, const float *a, const float *b, float *out);
+void  mo_log_add_range(uint64_t n, uint32_t a_first_bits, float b, int swap, float *out);
+void  mo_post_prob_n(uint64_t n, const float *s, float min_score, float *out);
+void  mo_post_prob_range(uint64_t n, uint32_t s_first_bits, float min_score, float *out);
 
 /* flat layout: flat[5*(i*(LY+1)+j)+s], 0<=i<=LX, 0<=j<=LY (flatmx.h:11-15) */
 void  mo_fwd(const mo_hmm *h, const uint8_t *X, uint32_t LX, const uint8_t *Y, uint32_t LY, float *flat);

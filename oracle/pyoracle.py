@@ -3,6 +3,7 @@
 ctypes bindings for the two CPU checkers:
   * Oracle  : oracle/liboracle.so      (our C restatement, oracle/muscle_oracle.c)
   * Ref     : oracle/_ref/libmuscle_ref.so (the unmodified reference + oracle/ref_probe.cpp)
+  * RefMath : oracle/_ref/libref_math.so   (the reference's LOG_ADD and posterior probability, many inputs)
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs import
 this module.  The product package muscle_b200/ never does.
 """
@@ -15,6 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ORACLE_SO = os.path.join(HERE, "liboracle.so")
 REF_SO = os.path.join(HERE, "_ref", "libmuscle_ref.so")
 REF_CLI = os.path.join(HERE, "_ref", "muscle")
+REF_MATH_SO = os.path.join(HERE, "_ref", "libref_math.so")
 
 ENTRY = np.dtype([("p", "<f4"), ("col", "<u4")])
 
@@ -60,7 +62,72 @@ def _seq(s):
 	return np.frombuffer(bytes(s), dtype=np.uint8).copy()
 
 
-class Oracle:
+def _bind_sweeps(L, prefix):
+	for f, args in (("log_add_n", [C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]),
+	  ("log_add_range", [C.c_uint64, C.c_uint32, C.c_float, C.c_int, C.c_void_p]),
+	  ("post_prob_n", [C.c_uint64, C.c_void_p, C.c_float, C.c_void_p]),
+	  ("post_prob_range", [C.c_uint64, C.c_uint32, C.c_float, C.c_void_p])):
+		fn = getattr(L, prefix + f)
+		fn.argtypes = args
+		fn.restype = None
+
+
+class _Sweeps:
+	"""LOG_ADD and the posterior probability of a score on many inputs (OpenMP): `_sw` is mo_ or ref_"""
+	_sw = None
+
+	def _f(self, name):
+		return getattr(self.lib, self._sw + name)
+
+	def log_add_n(self, a, b):
+		a = np.ascontiguousarray(a, np.float32)
+		b = np.ascontiguousarray(b, np.float32)
+		assert a.shape == b.shape
+		out = np.empty(a.size, np.float32)
+		self._f("log_add_n")(a.size, a.ctypes.data, b.ctypes.data, out.ctypes.data)
+		return out
+
+	def log_add_range(self, n, first_bits, b, swap=False):
+		"""LOG_ADD(a[k], b), or LOG_ADD(b, a[k]) when swap, for the floats a[k] of bits first_bits + k"""
+		out = np.empty(n, np.float32)
+		self._f("log_add_range")(n, first_bits & 0xffffffff, float(np.float32(b)), int(swap), out.ctypes.data)
+		return out
+
+	def post_prob_n(self, s, min_score):
+		s = np.ascontiguousarray(s, np.float32)
+		out = np.empty(s.size, np.float32)
+		self._f("post_prob_n")(s.size, s.ctypes.data, float(np.float32(min_score)), out.ctypes.data)
+		return out
+
+	def post_prob_range(self, n, first_bits, min_score):
+		out = np.empty(n, np.float32)
+		self._f("post_prob_range")(n, first_bits & 0xffffffff, float(np.float32(min_score)), out.ctypes.data)
+		return out
+
+
+def bit_mismatches(got, want, inputs, what, limit=16):
+	"""None when got and want hold the same float32 bits everywhere (never compared as floats: -0.0 == 0.0
+	and NaN != NaN); else a message with the count and the first `limit` offending inputs in hex.  inputs: an
+	int (element k came from the float of bits inputs + k) or a tuple of float32 arrays (the operands)."""
+	g = np.ascontiguousarray(got, np.float32).view(np.uint32)
+	w = np.ascontiguousarray(want, np.float32).view(np.uint32)
+	assert g.shape == w.shape, (g.shape, w.shape)
+	bad = np.flatnonzero(g != w)
+	if bad.size == 0:
+		return None
+	rows = []
+	for k in bad[:limit]:
+		if isinstance(inputs, (int, np.integer)):
+			ops = ["%08x" % ((int(inputs) + int(k)) & 0xffffffff)]
+		else:
+			ops = ["%08x" % int(np.asarray(x, np.float32).view(np.uint32)[k]) for x in inputs]
+		rows.append("(%s) -> %08x, want %08x" % (", ".join(ops), int(g[k]), int(w[k])))
+	return "%s: %d of %d differ; first: %s" % (what, bad.size, g.size, "; ".join(rows))
+
+
+class Oracle(_Sweeps):
+	_sw = "mo_"
+
 	def __init__(self, tables):
 		if not os.path.exists(ORACLE_SO):
 			build(ref=False)
@@ -76,6 +143,7 @@ class Oracle:
 		L.mo_sparse_from_post.restype = C.c_uint32
 		L.mo_all_pairs.restype = C.c_uint64
 		L.mo_free.argtypes = [C.c_void_p]
+		_bind_sweeps(L, "mo_")
 
 	def log_add(self, x, y):
 		return self.lib.mo_log_add(x, y)
@@ -301,6 +369,17 @@ class Ref:
 
 	def mpc(self, seqs):
 		return RefMPC(self, seqs)
+
+
+class RefMath(_Sweeps):
+	"""The reference's own LOG_ADD and posterior probability on many inputs (oracle/ref_math_probe.cpp)"""
+	_sw = "ref_"
+
+	def __init__(self):
+		if not os.path.exists(REF_MATH_SO):
+			raise FileNotFoundError(REF_MATH_SO + " (run `make -C oracle ref` where /root/reference exists)")
+		self.lib = C.CDLL(REF_MATH_SO)
+		_bind_sweeps(self.lib, "ref_")
 
 
 class RefMPC:
